@@ -10,13 +10,18 @@ whole attempts, 200x200 RGB-D render, host rewards AND the observation copied to
 hands it to its caller).  Extra objects on the same JSON line (not the headline): `configs` = BASELINE configs 3, 4, 5 as
 specified (SURVEY 8d; config 5 runs in a child process per rank), `qnet` = the a16 forward alone, `learner` = one learn() update.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--legs 3,4,5,qnet,learn]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--legs 3,4,5,qnet,learn] [--dump-outputs DIR]
 Under torchrun every rank owns one GPU and its own envs (weak scaling, no data-path collective).
+--dump-outputs DIR writes, after the timed steps, what the last timed step left for a caller of the engine (per-env state, results,
+status) as DIR/<name>.npy in float64; the inputs are seeded, so two builds run with the same arguments can be compared output for output.
+The tree is only read: the one thing compiled at run time (the fast oracle build of the CPU baseline) goes to a temporary directory.
 """
 import argparse
+import atexit
 import hashlib
 import json
 import os
+import shutil
 import subprocess
 import sys
 import tempfile
@@ -24,6 +29,7 @@ import time
 
 import numpy as np
 
+sys.dont_write_bytecode = True  # the tree may be read-only: no __pycache__ next to the sources
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
@@ -31,7 +37,7 @@ METRIC = "mujoco_substeps_per_sec"
 UNIT = "substeps/s"
 STATE_BYTES_PER_SUBSTEP = 2 * (50 + 44 + 44 + 14) * 8  # fp64 read+write of qpos, qvel, qacc_warmstart, 7 PID inputs, 7 targets (scene A)
 ENGINE_SO = os.path.join(ROOT, "mujoco_rl_ur5_b200", "csrc", "libgrasp_engine.so")
-ORACLE_FAST = os.path.join(ROOT, "oracle", "libgrasp_oracle_fast.so")
+ORACLE_FAST = os.path.join(tempfile.gettempdir(), "grasp_bench_oracle_%d" % os.getpid(), "libgrasp_oracle_fast.so")
 
 
 def measured_peak():
@@ -41,7 +47,7 @@ def measured_peak():
             return float(json.load(open(p))["hbm_gbs"]), "measured"
         except Exception:
             pass
-    return 6650.0, "fallback"
+    return 3350.0, "H100 SXM data sheet"
 
 
 def host_cores():
@@ -81,16 +87,24 @@ def lib_sha16(path=ENGINE_SO):
 
 
 def build_fast_oracle():
-    """-O3 -march=native -ffp-contract=fast build of the oracle, compiled on THIS machine (the optimistic CPU baseline)"""
+    """-O3 -march=native -ffp-contract=fast build of the oracle, compiled on THIS machine (the optimistic CPU baseline), in a temporary
+    directory outside the tree"""
     try:
-        subprocess.check_call(["make", "-s", "-C", os.path.join(ROOT, "oracle"), "-B", "fast"], stdout=subprocess.DEVNULL, stderr=subprocess.DEVNULL)
+        d = os.path.dirname(ORACLE_FAST)
+        os.makedirs(d, exist_ok=True)
+        atexit.register(shutil.rmtree, d, True)  # removed when this process ends (the oracle workers it starts end before it)
+        for f in ("grasp_oracle.c", "orc_math.h"):
+            with open(os.path.join(ROOT, "oracle", f), "rb") as src, open(os.path.join(d, f), "wb") as dst:
+                dst.write(src.read())
+        subprocess.check_call(["make", "-s", "-C", d, "-f", os.path.join(ROOT, "oracle", "Makefile"), "-B", "fast"], stdout=subprocess.DEVNULL,
+                              stderr=subprocess.DEVNULL)
         return os.path.exists(ORACLE_FAST)
     except Exception:
         return False
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     Q = "index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
 
@@ -292,6 +306,17 @@ def run_config5_child(args):
     print(json.dumps(out), flush=True)
 
 
+def dump_outputs(out_dir, eng):
+    """what the timed path (BatchedEngine.grasp + run_async) leaves for its caller after the last timed step, float64 .npy files"""
+    os.makedirs(out_dir, exist_ok=True)
+    qpos, qvel = eng.get_state()
+    result, steps, reward, total = eng.results()
+    arrays = {"qpos": qpos, "qvel": qvel, "result": result, "steps": steps, "reward": reward, "substeps": total, "busy": eng.busy(),
+              "status": eng.status(), "grasp_info": eng.grasp_info()}
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a.cpu().numpy().astype(np.float64))
+
+
 def run_ours(args):
     import torch
     import torch.distributed as dist
@@ -312,7 +337,7 @@ def run_ours(args):
     env.reset()
     gen = torch.Generator(device=dev)
     gen.manual_seed(30000 + rank)
-    flush = torch.empty(256 * 1024 * 1024 // 4, dtype=torch.float32, device=dev)  # > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024 // 4, dtype=torch.float32, device=dev)  # > 50 MB L2
 
     def assign_idle():
         idle = (eng.busy() == 0)
@@ -361,6 +386,8 @@ def run_ours(args):
         kern_evs.append((b, c))
     barrier()
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, eng)
     ms = sum(a.elapsed_time(c) for a, c in evs)
     kern_ms = sum(b.elapsed_time(c) for b, c in kern_evs)
     sub1 = env.total_substeps()
@@ -404,7 +431,7 @@ def run_ours(args):
     except Exception:
         pass
 
-    # ---- a16: Q-network forward (bf16 tcgen05) alone; extra object, not the headline
+    # ---- a16: Q-network forward (bf16 wgmma) alone; extra object, not the headline
     qinfo = None
     qf = None
     if "qnet" in legs or "4" in legs:
@@ -428,10 +455,10 @@ def run_ours(args):
         barrier()
         qms = q0.elapsed_time(q1) / args.qnet_reps
         tf = nimg * 41.99424e9 / (qms * 1e-3) / 1e12
-        pk = float(peaks.get("bf16_tflops_sustained", 1400.0))
+        pk = float(peaks.get("bf16_tflops_sustained", 989.0))
         qinfo = {"images": nimg, "chunk": args.qnet_chunk, "ms_per_batch": qms, "images_per_s": nimg / (qms * 1e-3), "tflops": tf,
                  "roofline": {"bound": "tensor", "achieved": tf, "peak": pk, "unit": "TFLOP/s", "frac": tf / pk,
-                              "note": "41.99 GFLOP per 200x200 image (SURVEY 8d); peak = " + ("measured sustained cuBLAS bf16" if peaks else "fallback")},
+                              "note": "41.99 GFLOP per 200x200 image (SURVEY 8d); peak = " + ("measured sustained cuBLAS bf16" if peaks else "H100 SXM data sheet, dense bf16")},
                  "kernels_per_batch": (qf.launches - l_q0) // max(args.qnet_reps, 1)}
         envq.close()
         del envq, sub
@@ -468,7 +495,7 @@ def run_ours(args):
         linfo = {"batch_per_gpu": lb, "ms_per_update": lms, "updates_per_s": 1e3 / lms, "transitions_per_s": world * lb * 1e3 / lms, "tflops_per_gpu": ltf,
                  "kernels_per_update": (learner.launches - l_l0) // max(args.qnet_reps, 1), "loss": loss_l,
                  "collective": ("all_reduce of %.1f MB fp32 gradients over %d ranks (NCCL)" % (learner.grad.numel() * 4 / 1e6, world)) if use_pg else None,
-                 "note": "QNetLearner.learn_step: forward (tcgen05) with batch-statistics BN, gather-BCE, dgrad (tcgen05), wgrad (CUDA-core tiles), Adam; "
+                 "note": "QNetLearner.learn_step: forward (wgmma) with batch-statistics BN, gather-BCE, dgrad (wgmma), wgrad (wgmma), Adam; "
                          "includes the loss .item() read like the reference"}
         del learner, st, ac, rw
 
@@ -510,12 +537,12 @@ def run_ours(args):
         t0 = time.perf_counter()
         rew = 0
         for _ in range(args.leg_steps):
-            act, _ = agent.greedy(obs)           # obs -> state (device) -> tcgen05 forward of all images -> arg-max; actions stay on the GPU
+            act, _ = agent.greedy(obs)           # obs -> state (device) -> wgmma forward of all images -> arg-max; actions stay on the GPU
             obs, r, _, _ = e4.step(act)
             rew += int(r.sum())
         torch.cuda.synchronize()
         n4s, s4 = aggregate(e4.total_substeps() - n0, time.perf_counter() - t0)
-        configs["4"] = {"workload": f"BASELINE config 4: {n4} envs/GPU (x{world} GPUs), scene A1, every step = Q-net forward (bf16 tcgen05, random-init "
+        configs["4"] = {"workload": f"BASELINE config 4: {n4} envs/GPU (x{world} GPUs), scene A1, every step = Q-net forward (bf16 wgmma, random-init "
                                     f"weights torch.manual_seed(0), chunks of {args.qnet_chunk}) over ALL {n4} observations -> greedy pixel/rotation -> whole grasp "
                                     "attempt -> RGB-D render",
                         "value": n4s / s4, "unit": UNIT, "steps": args.leg_steps, "qnet_images_per_step": world * n4,
@@ -630,6 +657,7 @@ def main():
     ap.add_argument("--qnet-reps", type=int, default=3)
     ap.add_argument("--scene-b-envs", type=int, default=1024, help="environments per GPU of the config 5 leg")
     ap.add_argument("--scene-b-steps", type=int, default=1, help="timed BatchedGraspEnv.step calls (full grasp attempts) of the config 5 leg")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR", help="write the outputs of the last timed step to DIR/<name>.npy")
     ap.add_argument("--ref-step-seconds", type=float, default=3.0, help="--impl reference: wall-time budget per worker and step")
     ap.add_argument("--oracle-leg", type=float, default=None, help=argparse.SUPPRESS)
     ap.add_argument("--config5-child", type=int, default=None, help=argparse.SUPPRESS)

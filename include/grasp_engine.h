@@ -1,4 +1,4 @@
-/* grasp_engine.h — C-ABI of the B200 batched grasp-simulation engine (libgrasp_engine.so).
+/* grasp_engine.h — C-ABI of the H100 batched grasp-simulation engine (libgrasp_engine.so).
  *
  * The reference has no FFI layer: its boundary is two Python classes (GraspEnv, MJ_Controller) that poke
  * mujoco_py attributes.  Each entry point below names the reference interface it stands in for (file:line in
@@ -33,7 +33,7 @@ enum { GE_MOVE_RUNNING = 0, GE_MOVE_SUCCESS = 1 /* "success" */, GE_MOVE_MAXSTEP
 enum { GE_STATUS_CONTACT_OVERFLOW = 1, GE_STATUS_NONFINITE = 2, GE_STATUS_SOLVER_MAXITER = 4 };
 
 const char* ge_last_error(void);
-/* library / build identification: returns e.g. "grasp_engine 0.1 sm_100a fp64" */
+/* library / build identification: returns e.g. "grasp_engine 0.1 sm_90a fp64" */
 const char* ge_version(void);
 
 /* mujoco_py.load_model_from_path + MjSim (MujocoController.py:33-36) + MJ_Controller.create_lists (:136-254):

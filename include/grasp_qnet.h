@@ -18,9 +18,12 @@ const char* gq_last_error(void);
 const char* gq_version(void);
 
 /* nn.Conv2d(Cin, Cout, kernel_size=ks, padding=ks/2, stride=1) for ks in {1,3}, Cin and Cout multiples of 64 (conv3x3: Modules.py:145-156;
- * BasicBlock.conv3 1x1 with bias: :126).  tcgen05 implicit GEMM.  x [B,H,W,Cin] bf16, w [Cout][ks*ks][Cin] bf16, bias [Cout] f32 or NULL,
+ * BasicBlock.conv3 1x1 with bias: :126).  wgmma implicit GEMM.  x [B,H,W,Cin] bf16, w [Cout][ks*ks][Cin] bf16, bias [Cout] f32 or NULL,
  * y [B,H,W,Cout] f32.  If stats != NULL, stats[B][Cout][2] f32 := per-image (sum, sum of squares) of y over H*W, computed
- * deterministically through `partials`, a scratch buffer of B * ceil(H*W/128) * 4 * Cout * 2 floats. */
+ * deterministically through `partials`, a scratch buffer of gq_conv_partials_floats(B, H, W, Cout) floats. */
+/* size in floats of the `partials` scratch buffer gq_conv_tc needs for per-image statistics: one (sum, sum of squares) row of Cout per
+ * consumer warp and 128-pixel tile of every image = B * ceil(H*W/128) * 8 * Cout * 2 */
+size_t gq_conv_partials_floats(int B, int H, int W, int Cout);
 int gq_conv_tc(const void* x, const void* w, const float* bias, float* y, float* stats, float* partials, int B, int H, int W, int Cin, int Cout, int ks,
                void* stream);
 /* Tail of BasicBlock.forward (Modules.py:136-142: `out = bn2(conv2(out)); identity = conv3(x); out += identity; out = relu(out)`) with the

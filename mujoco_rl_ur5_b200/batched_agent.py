@@ -2,7 +2,7 @@
 
 Reference: Grasping_Agent_multidiscrete.py — `greedy` (:284-299) = transform_observation (:301-368) -> policy_net (:295) ->
 flat arg-max -> transform_action (:381-386); `epsilon_greedy` (:232-282) mixes in uniformly random table pixels.
-Here: gq_obs_to_state -> tcgen05 Q-network forward -> gq_argmax, all kernels of libgrasp_qnet.so; the result is an int32
+Here: gq_obs_to_state -> wgmma Q-network forward -> gq_argmax, all kernels of libgrasp_qnet.so; the result is an int32
 [N,2] tensor (pixel index, rotation index) that BatchedGraspEnv.step accepts without leaving the GPU (BASELINE config 4).
 The learner (replay buffer, BCE loss, Adam; :388-446) is a SURVEY 8(f) "next" row and is not part of this class.
 """

@@ -1,4 +1,4 @@
-"""Drop-in `gym_grasper` package: same registration as the reference (gym_grasper/__init__.py:4-7), B200-backed env."""
+"""Drop-in `gym_grasper` package: same registration as the reference (gym_grasper/__init__.py:4-7), H100-backed env."""
 from gym.envs.registration import register
 
 from .version import VERSION as __version__  # noqa: F401

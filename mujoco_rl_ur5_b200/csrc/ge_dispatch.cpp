@@ -51,7 +51,7 @@ static thread_local int g_last_variant = 0;
 extern "C" {
 
 const char* ge_last_error(void) { return g_last_variant ? ge_last_error_hbm() : ge_last_error_smem(); }
-const char* ge_version(void) { return "grasp_engine 0.2 sm_100a fp64 warp-per-env (variants: shared-memory workspace, HBM workspace)"; }
+const char* ge_version(void) { return "grasp_engine 0.2 sm_90a fp64 warp-per-env (variants: shared-memory workspace, HBM workspace)"; }
 
 int ge_create(const void* blob, size_t nbytes, int n_envs, int device, void* stream, ge_handle* out) {
   if (!out) return GE_ERR_ARG;

@@ -52,7 +52,7 @@ __device__ __forceinline__ void jac_column(const double* c, int dim, const doubl
 // are disjoint, so the warps never touch the same entry)
 // The owner is chosen per Hessian build by longest-processing-time-first over the islands' cubic cost (build_hessian) and kept in slot 1
 // of the representative's list row: with `island % GE_NW` one warp regularly held the two largest islands of a pile while the others
-// idled at the next barrier (r02f ncu: barrier = 40-47 % of the stall cycles in build_hessian / cholesky_solve).
+// idled at the next barrier.
 __device__ __forceinline__ int island_owner(const int* island, const int* tlist, int t) { return tlist[island[t] * 16 + 1]; }
 // per-tree bookkeeping of one Hessian build: block offset (of the tree's own block, or of its island's block) and, for coupled trees,
 // the tree's first row inside the island block
@@ -268,7 +268,7 @@ __device__ __noinline__ void build_hessian(double* ws, int* wi, int ncon, int ns
     }
     // The contact touches n dofs (12 for two free bodies), a warp has 32 lanes: P = 32 / n lanes share one row of the n x n update, lane
     // (r, p) takes the columns p, p + P, ...  Every entry still receives exactly one addition per contact, computed in the same order, so
-    // the result does not depend on P.  (r02g piled-pile capture: this loop was 19 K of the 55 K warp instructions of a Hessian build.)
+    // the result does not depend on P.
     const int P = n > 0 && n <= 16 ? 32 / n : 1, r_ = n > 0 ? wl % n : 0, p_ = n > 0 ? wl / n : 0;
     const bool act = n > 0 && p_ < P && r_ < n;
     mydof = __shfl_sync(FULL, mydof, r_);
@@ -317,8 +317,7 @@ __device__ __noinline__ void build_hessian(double* ws, int* wi, int ncon, int ns
 // lo + nt - 1) inside an 8-lane group, entirely in REGISTERS: lane l loads row l of the block once (static register indices, the loops
 // are fully unrolled), the factorisation exchanges pivots / column entries through shuffles, nothing is written back to the matrix
 // (the factor is used exactly once).  Rows l >= nt are padded with the identity.  x[lo + l] := sign * (H_block^-1 g)[l].
-// (r02: the shared-memory version spent ~1000 instructions per block in packed-index arithmetic, LDS/STS and three __syncwarp per
-// column; mass_block_solve + the group path of cholesky_solve were 22 % of k_run's time.)
+// (A shared-memory version spends most of its instructions in packed-index arithmetic, LDS/STS and three __syncwarp per column.)
 __device__ __noinline__ void group_chol_solve(const double* Hb, int lo, int nt, int l, unsigned gmask, const double* g_, double* x, double sign) {
   const int row = lo + l;
   const bool mine = l < nt;

@@ -78,6 +78,8 @@ struct EnvArrays {
   long long* substeps;            // [N]
   int* busy_count;                // [1]
   int* lock;                      // [N] 1 while a warp of k_run holds the env (dynamic env -> warp assignment)
+  int* owed;                      // [N] visits of the env drawn in this launch and not yet run (k_run: a drawer never drops a visit)
+  int* done;                      // [N] iterations the env has been given in this launch (reset before every launch)
   unsigned long long* ticket;     // [1] monotonically increasing task counter of k_run (never reset: launches subtract their base)
   double* gws;                    // [N, hfull] Hessian overflow rows (big-scene build when hcap < hfull), else NULL
 };

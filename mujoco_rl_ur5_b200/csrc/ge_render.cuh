@@ -178,9 +178,9 @@ __global__ void __launch_bounds__(RTILE * RTILE) k_render(const double* gframes,
   __syncthreads();
   // The tile lists the geoms whose screen box (k_render_fk) meets its pixel range, and keeps the box so that each pixel also skips the
   // geoms whose box it lies outside of.  The boxes only drop geoms no ray of the tile / pixel can hit: the image is the same as with
-  // the full list.  r01 culled with the tile's bounding cone against bounding spheres: the table top, legs and bin walls (spheres of
-  // 0.35-0.5 m) passed for every tile, 6.1 listed geoms per tile in the 6-object scene against 2.7 now; r02j computed the boxes here,
-  // per tile, and spent the gain at this barrier (36 busy threads of 256: `barrier` 3.0 cycles per issue) - now once per env.
+  // the full list.  A bounding-cone test against bounding spheres alone lets the table top, legs and bin walls
+  // (spheres of 0.35-0.5 m) through for every tile.  The boxes are computed once per env: computed here, per tile, most threads would
+  // wait at this barrier.
   {
     const int c0i = tx * RTILE, c1i = min(W, c0i + RTILE), r0i = ty * RTILE, r1i = min(H, r0i + RTILE);
     const short4* gb = gbox + (size_t)env * m.ngeom;

@@ -1,5 +1,5 @@
 // libgrasp_engine.so — C-ABI (include/grasp_engine.h) + kernels of the batched grasp-simulation engine.
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -lineinfo -shared -Xcompiler -fPIC (see __graft_entry__.build()).
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -shared -Xcompiler -fPIC (see __graft_entry__.build()).
 #include "ge_variant.h"  // must come first: renames the namespace and the C entry points of this build variant
 
 #include <cuda_runtime.h>
@@ -23,17 +23,19 @@ static int fail(int code, const char* fmt, const char* a = "") { snprintf(g_err,
 #define CK(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) return fail(GE_ERR_CUDA, "CUDA error: %s", cudaGetErrorString(e_)); } while (0)
 
 extern "C" const char* ge_last_error(void) { return g_err; }
-extern "C" const char* ge_version(void) { return GE_NW > 1 ? "grasp_engine 0.3 sm_100a fp64 CTA-per-env (4 warps, workspace: shared memory, Hessian overflow: HBM)" : "grasp_engine 0.3 sm_100a fp64 warp-per-env (workspace: shared memory)"; }
+extern "C" const char* ge_version(void) { return GE_NW > 1 ? "grasp_engine 0.3 sm_90a fp64 CTA-per-env (4 warps, workspace: shared memory, Hessian overflow: HBM)" : "grasp_engine 0.3 sm_90a fp64 warp-per-env (workspace: shared memory)"; }
 
 // ------------------------------------------------------------------------------------------------ kernels
 // Sub-step kernel: one warp per environment, environments handed to warps DYNAMICALLY.
 // A launch gives every environment a budget of `nsub` iterations of the reference control loop (PID -> mj_step, including the
 // movement / grasp-program transitions), split into visits of `quota` iterations.  Task t of a launch = (visit t / n_env, env t % n_env);
-// a warp that has no environment takes the next task from a global counter, skips it if the environment is idle or another warp
-// still holds it (per-env lock, never waited for), otherwise loads the env's state rows into its shared-memory slice, runs the
-// visit and writes the rows back.  The grid is persistent (<= the resident CTAs), so 4096 envs on 1184 warp slots cost 13.84 -> 14
-// rounds of 64 iterations instead of 3.46 -> 4 rounds of 256, finished or idle environments stop costing anything, and the tail
-// of a batch of unequal grasp attempts is spread over all SMs.  Arithmetic per env is unchanged: the state crosses HBM in full
+// a warp that has no environment takes the next task from a global counter, skips it if the environment is idle, otherwise records
+// the visit as owed to the env and runs it if it can take the env's lock (never waited for: a warp still holding the env runs the owed
+// visit after its own one, see env_take).  A visit loads the env's state rows into the warp's shared-memory slice, runs
+// min(quota, iterations the env has left in this launch) and writes the rows back.  So every busy env is given exactly `nsub`
+// iterations per launch whatever the timing, and the result of a launch does not depend on which warp ran which visit.  The grid is persistent (<= the resident CTAs), so envs beyond the
+// resident warp slots cost rounds of `quota` iterations instead of whole launches, finished or idle environments stop costing anything,
+// and the tail of a batch of unequal grasp attempts is spread over all SMs.  Arithmetic per env is unchanged: the state crosses HBM in full
 // fp64 between visits, so a trajectory does not depend on how its iterations were cut.
 // A CTA holds `blockDim.y` warps; they meet at one barrier per iteration (+ the stage barriers) so that the warps of an SM walk
 // the (large) sub-step code roughly together and share instruction-cache lines.
@@ -85,11 +87,27 @@ __device__ __forceinline__ unsigned long long group_bcast_u64(unsigned long long
   return r;
 #endif
 }
+// lane 0 of a group, owed visits of env e pending: take the env's lock and one owed visit of a busy env with iterations left; 0 when the
+// lock is held elsewhere (its holder takes the owed visits when it lets go) or nothing is owed.  An owed visit of an env that has gone
+// idle or used its budget is consumed without running.  Owed counts may be transiently negative while a taker undoes its claim.
+__device__ int env_take(const EnvArrays& E, int e, int nsub) {
+  while (atomicCAS(E.lock + e, 0, 1) == 0) {
+    __threadfence();
+    const bool owed = atomicSub(E.owed + e, 1) > 0;
+    if (!owed) atomicAdd(E.owed + e, 1);  // undo: nothing was owed
+    else if (env_is_busy(E, e) && __ldcg(E.done + e) < nsub) return 1;
+    __threadfence();
+    atomicExch(E.lock + e, 0);
+    __threadfence();
+    if (atomicAdd(E.owed + e, 0) <= 0) return 0;  // a visit owed after the release is taken by the one who drew it, or here
+  }
+  return 0;
+}
 // blockDim = (GE_LANES, envs per CTA): threadIdx.x is the lane inside the group that owns one environment (a warp; a whole CTA of
 // GE_NW warps in the big-scene build, where blockDim.y = 1)
 // Register budget.  Warp-per-env build: `__launch_bounds__(256)` alone makes ptxas settle on 128 registers per thread (stack 1616 B); told
 // that one 256-thread CTA per SM is enough it takes 246 (stack 1296 B), which still fits the 2 x 128-thread CTAs the shared memory allows
-// (65 536 registers per SM) - r02g: 3.93 -> 4.20 M sub-steps/s at 4096 envs (-DGE_V0_CAP_REGS restores the old budget).
+// (65 536 registers per SM; -DGE_V0_CAP_REGS restores the 128-register budget).
 // CTA-per-env build: two CTAs per SM is what the workspace allows; the bound keeps the register file from undercutting it.
 #if GE_NW > 1
 #define GE_RUN_BOUNDS __launch_bounds__(GE_LANES, 2)
@@ -109,8 +127,8 @@ __global__ void GE_RUN_BOUNDS k_run(EnvArrays E, int n_env, int nsub, int quota,
   double* ws = smem + (size_t)threadIdx.y * (L.total_bytes / 8);
   int* wi = (int*)(ws + L.total_doubles);
   EnvRegs r;
-  int env = -1, left = 0;
-  bool exhausted = false, running = false;
+  int env = -1, left = 0, visit_len = 0;
+  bool exhausted = false, running = false;  // running: the group has a loaded visit of `env` in progress
   for (;;) {
     // ---- a group without an environment takes tasks until it finds a busy, unlocked environment (or the launch has none left)
     while (env < 0 && !exhausted) {
@@ -118,24 +136,27 @@ __global__ void GE_RUN_BOUNDS k_run(EnvArrays E, int n_env, int nsub, int quota,
       if (lane == 0) t = atomicAdd(E.ticket, 1ULL) - ticket_base;
       t = group_bcast_u64(t, lane);
       if (t >= total) { exhausted = true; break; }
-      const int e = (int)(t % (unsigned long long)n_env), v = (int)(t / (unsigned long long)n_env);
+      const int e = (int)(t % (unsigned long long)n_env);
       // ONE thread looks at the env's flags and takes the lock, the group follows its verdict: the flags change under our feet when
       // another group finishes a visit of this env, and threads that read them separately (the four warps of a CTA-per-env group do
-      // so at different times) would part ways - r02d: illegal instruction / illegal address at >= 300 envs
+      // so at different times) would part ways
       int got = 0;
-      if (lane == 0 && env_is_busy(E, e) && atomicCAS(E.lock + e, 0, 1) == 0) {
-        // an earlier visit of this env still running elsewhere fails the CAS: this visit is dropped, never waited for
+      if (lane == 0 && env_is_busy(E, e)) {
+        atomicAdd(E.owed + e, 1);
         __threadfence();
-        if (env_is_busy(E, e)) got = 1;
-        else atomicExch(E.lock + e, 0);
+        got = env_take(E, e, nsub);
       }
       got = group_bcast_int(got, lane);
       if (!got) continue;
+      env = e;
       __threadfence();
       if (GE_NW > 1 && lane == 0) g_hovf = E.gws ? E.gws + (size_t)e * L.hfull : nullptr;  // this env's Hessian overflow row
-      env_load(E, e, ws, lane, r);
-      env = e; running = true;
-      left = nsub - v * quota < quota ? nsub - v * quota : quota;
+    }
+    if (env >= 0 && !running) {  // a visit was taken (drawn above, or owed to the env this group just stored): load and run it
+      env_load(E, env, ws, lane, r);
+      const int d = __ldcg(E.done + env);
+      left = visit_len = nsub - d < quota ? nsub - d : quota;
+      running = true;
     }
 #if GE_NW == 1
     __syncwarp();
@@ -166,10 +187,19 @@ __global__ void GE_RUN_BOUNDS k_run(EnvArrays E, int n_env, int nsub, int quota,
       while (!r.c.active && r.p.phase != PH_NONE) { if (!prog_advance(r.p, r.c, ws, lane, base, r.info, &r.reward)) break; }
       gsync();
       env_store(E, env, ws, lane, r);
+      if (lane == 0) E.done[env] = __ldcg(E.done + env) + visit_len;
       __threadfence();
       gsync();
-      if (lane == 0) atomicExch(E.lock + env, 0);
-      env = -1;
+      // let go of the env, then run a visit owed to it meanwhile (its drawer found the lock held and left it to us)
+      int again = 0;
+      if (lane == 0) {
+        atomicExch(E.lock + env, 0);
+        __threadfence();
+        if (atomicAdd(E.owed + env, 0) > 0) again = env_take(E, env, nsub);
+      }
+      again = group_bcast_int(again, lane);
+      running = false;
+      if (!again) env = -1;
     }
   }
 }
@@ -602,9 +632,9 @@ extern "C" int ge_create(const void* model_blob, size_t nbytes, int n_envs, int 
   AL(E.cmd_mask, int, N); AL(E.cmd_maxsteps, int, N); AL(E.cmd_steps, int, N); AL(E.cmd_result, int, N); AL(E.cmd_active, int, N); AL(E.cmd_tol, double, N);
   AL(E.prog_phase, int, N); AL(E.prog_rot, int, N); AL(E.prog_grasp, int, N); AL(E.prog_aux, int, N); AL(E.prog_info, int, N * 12);
   AL(E.prog_coords, double, N * 3); AL(E.prog_table, double, N); AL(E.reward, unsigned char, N); AL(E.status, int, N); AL(E.substeps, long long, N);
-  AL(E.busy_count, int, 1); AL(E.lock, int, N); AL(E.ticket, unsigned long long, 1);
+  AL(E.busy_count, int, 1); AL(E.lock, int, N); AL(E.owed, int, N); AL(E.done, int, N); AL(E.ticket, unsigned long long, 1);
   h->ticket_base = 0;
-  h->quota = 32;  // r02c sweep at 4096 envs: 32 -> 3.89 M, 64 -> 3.81 M, 128 -> 3.59 M, 256 (= one visit per launch) -> 3.24 M sub-steps/s
+  h->quota = 32;  // iterations per visit; H100, 4096 envs: see DESIGN.md section 4 (GE_QUOTA overrides)
   if (const char* ev = getenv("GE_QUOTA")) { int v = atoi(ev); if (v >= 1) h->quota = v; }
   {
     int per_sm = 0, sms = 0;
@@ -645,7 +675,7 @@ extern "C" int ge_destroy(ge_handle h) {
   EnvArrays& E = h->E;
   void* ptrs[] = {E.qpos, E.qvel, E.qaccws, E.ctl, E.cmd_mask, E.cmd_maxsteps, E.cmd_steps, E.cmd_result, E.cmd_active, E.cmd_tol, E.prog_phase,
                   E.prog_rot, E.prog_grasp, E.prog_aux, E.prog_info, E.prog_coords, E.prog_table, E.reward, E.status, E.substeps, E.busy_count,
-                  h->d_nout, h->d_dbg, h->dblob, E.gws, E.lock, E.ticket};
+                  h->d_nout, h->d_dbg, h->dblob, E.gws, E.lock, E.owed, E.done, E.ticket};
   for (void* p : ptrs) cudaFree(p);
   render_free(h->rctx);
   delete h;
@@ -739,6 +769,7 @@ extern "C" int ge_run_async(ge_handle h, int substeps) {
   int ctas = (h->n_envs + h->wpb - 1) / h->wpb;
   if (ctas > h->max_ctas) ctas = h->max_ctas;  // persistent grid: environments are handed to warps dynamically
   int quota = h->quota < substeps ? h->quota : substeps;
+  CK(cudaMemsetAsync(h->E.done, 0, sizeof(int) * h->n_envs, h->stream));
   k_run<<<ctas, blk, (size_t)h->wpb * h->ws_smem, h->stream>>>(h->E, h->n_envs, substeps, quota, h->ticket_base, h->base_pos[0], h->base_pos[1],
                                                                 h->base_pos[2], h->stage_sync);
   // every warp takes tasks until it has drawn one beyond the launch's range: n_env * visits real tasks + one overshoot per warp

@@ -2,10 +2,10 @@
 // Perception_Module :159-193 + Grasping_Module_multidiscrete :243-287, BasicBlock :92-142) over a batch of environments.
 //
 // bf16 activations (NHWC) and weights, fp32 accumulation.  The 3x3 / 1x1 convolutions with Cin >= 64 (>99.9 % of the MACs) run
-// as implicit GEMMs on the 5th-generation tensor cores: tcgen05.mma (kind::f16, M=128, N=64/128, K=16) with the accumulator in
-// TMEM, operands gathered into shared memory in the canonical K-major no-swizzle core-matrix layout, completion tracked with
-// tcgen05.commit -> mbarrier, epilogue through tcgen05.ld.  BatchNorm uses per-image batch statistics because the reference
-// never puts the policy net in eval() and forwards one image at a time (SURVEY 3.4, quirk Q9).
+// as implicit GEMMs on the Hopper tensor cores: both operands are brought into 128-byte-swizzled K-major shared-memory tiles by TMA
+// (an im2col-mode map for the activations, a tiled map for the weights), completion tracked with mbarrier transaction counts, and
+// two consumer warpgroups multiply them with wgmma.mma_async (m64 x N x k16, accumulator in registers).  BatchNorm uses per-image
+// batch statistics because the reference never puts the policy net in eval() and forwards one image at a time (SURVEY 3.4, quirk Q9).
 //
 // C-ABI: see include/grasp_qnet.h.  No CPU fallback.
 #include <cuda.h>  // CUtensorMap (types only; the encoder is fetched with cudaGetDriverEntryPoint, libcuda is not linked)
@@ -17,7 +17,6 @@
 #include <string.h>
 
 #include "../../include/grasp_qnet.h"
-#include "qnet_plan.h"
 
 typedef __nv_bfloat16 bf16;
 
@@ -37,80 +36,10 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
                  : "=r"(done) : "r"(addr), "r"(parity) : "memory");
   }
 }
-__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory"); }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem]^T ; single-thread issue
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-               ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-// 32 lanes x 32 consecutive fp32 columns: thread t of the warp receives row (lane base + t)
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float* v) {
-  uint32_t r[32];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]),
-        "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]),
-        "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 32; i++) v[i] = __uint_as_float(r[i]);
-}
-// shared-memory matrix descriptor, K-major, no swizzle: core matrix = 8 rows x 16 B stored contiguously (128 B);
-// LBO = byte distance between the two 16-byte K-chunks of one MMA, SBO = byte distance between 8-row groups (kept for reference;
-// the convolution uses the 128-byte-swizzled layout below)
-__device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr >> 4) & 0x3fff);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3fff) << 16;
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3fff) << 32;
-  d |= (uint64_t)1 << 46;  // descriptor version (Blackwell)
-  return d;                // base offset 0, lbo mode 0, layout type 0 = SWIZZLE_NONE
-}
-// shared-memory matrix descriptor, K-major, SWIZZLE_128B: one tile row = 128 contiguous bytes (64 bf16 along K) whose eight 16-byte
-// chunks are XOR-ed with (row % 8); 8 rows form a 1024-byte atom (SBO), the tile base is 1024-byte aligned.  A K-step of 16
-// elements advances the start address by 32 bytes inside the atom.
-__device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t saddr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr >> 4) & 0x3fff);
-  d |= (uint64_t)1 << 16;            // leading byte offset: unused for swizzled K-major
-  d |= (uint64_t)(1024 >> 4) << 32;  // stride byte offset: 8 rows x 128 B
-  d |= (uint64_t)1 << 46;            // descriptor version (Blackwell)
-  d |= (uint64_t)2 << 61;            // layout type SWIZZLE_128B
-  return d;
-}
-// instruction descriptor kind::f16: D = F32, A = B = BF16, both K-major, shape M x N (K = 16)
-__host__ __device__ constexpr uint32_t make_idesc(int M, int N) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-
-// ------------------------------------------------------------------------------------------------ implicit-GEMM convolution on tcgen05
-// x  [B,H,W,Cin] bf16 (NHWC), w [Cout][ks*ks][Cin] bf16, y [B,H,W,Cout] f32 (+ bias), stats [B,Cout,2] f32 += (sum, sum of squares)
-// grid (ceil(H*W/128), Cout/BLOCK_N, B), 128 threads.  One CTA = 128 output pixels x BLOCK_N output channels of one image.
-#define BM 128
-#define BK 64
-// 16-byte asynchronous global -> shared copy (LDGSTS); src_bytes = 0 writes zeros (convolution padding, rows past the image)
-__device__ __forceinline__ void cp_async16(void* dst_smem, const void* src, uint32_t src_bytes) {
-  asm volatile("cp.async.ca.shared.global [%0], [%1], 16, %2;" ::"r"(smem_u32(dst_smem)), "l"(src), "r"(src_bytes) : "memory");
-}
-__device__ __forceinline__ void cp_async16_s(uint32_t dst_smem_addr, const void* src, uint32_t src_bytes) {
-  asm volatile("cp.async.ca.shared.global [%0], [%1], 16, %2;" ::"r"(dst_smem_addr), "l"(src), "r"(src_bytes) : "memory");
-}
-// TMA: one thread copies a whole [rows x 64 bf16] box of a 2-D tensor into a 128-byte-swizzled shared-memory tile; completion is
-// reported to the mbarrier as transferred bytes (complete_tx), so the same "full" barrier collects the cp.async arrivals and the TMA
+// TMA: one thread copies a whole box into a 128-byte-swizzled shared-memory tile; completion is reported to the mbarrier as
+// transferred bytes (complete_tx)
 __device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
 }
@@ -118,287 +47,128 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst_smem_addr, const CUtens
   asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
                ::"r"(dst_smem_addr), "l"((uint64_t)tmap), "r"(x), "r"(y), "r"(smem_u32(bar)) : "memory");
 }
-// .cg: cache in L2 only (weight tiles are read once per CTA; keeping them out of L1 leaves it to the activation rows the 9 taps re-read)
-__device__ __forceinline__ void cp_async16_cg(uint32_t dst_smem_addr, const void* src) {
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst_smem_addr), "l"(src) : "memory");
-}
-// Column sums of a 32 x 32 tile held one row per lane (v[c] = element (lane, c)): on return lane j holds sum_lanes v[j].
-// Recursive halving: at distance s the lanes with bit s set keep the upper s columns of what they still hold and hand the lower s to
-// their partner (and vice versa), so 16 + 8 + 4 + 2 + 1 = 31 shuffles replace 32 x 5; the summation tree is fixed (deterministic).
-__device__ __forceinline__ float warp_colsum32(float (&v)[32], int lane) {
-#pragma unroll
-  for (int s = 16; s >= 1; s >>= 1) {
-    const bool up = (lane & s) != 0;
-#pragma unroll
-    for (int k = 0; k < s; k++) {
-      const float send = up ? v[k] : v[k + s];
-      const float keep = up ? v[k + s] : v[k];
-      v[k] = keep + __shfl_xor_sync(0xffffffffu, send, s);
-    }
-  }
-  return v[0];
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-// arrive on the mbarrier once all cp.async issued so far by this thread have landed (does not bump the expected count)
-__device__ __forceinline__ void cp_async_mbar_arrive(uint64_t* bar) {
-  asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-
-// ---- non-persistent convolution kernel (GQ_PERSIST=0; the default until r02a, kept as the A/B partner of the persistent TMA kernel
-// below and as the path for drivers without cuTensorMapEncodeIm2col).  Same tiling, shared-memory layout, barrier protocol and MMA
-// issue as the first version of round 1 (removed in r02); what changed is what the ncu capture of v1 showed to be the limit (profiles/r01h_conv_tc_ncu_summary.txt: tensor pipe 17-23 % active,
-// issue slots 30-44 % busy with 1.25 resident warps per scheduler = the four producer warps executing ~700 instructions per k-step):
-//  * producer address arithmetic is hoisted out of the k-loop: every thread's 8 A rows and BLOCK_N/16 B rows are an arithmetic
-//    progression in global memory (row stride 16 pixels / 16 output channels) and in shared memory (2048 B: 16 rows x 128 B, the
-//    128-byte swizzle term depends on row % 8 only and is therefore the same for all rows of a thread); the zero-padding test of
-//    each (row, tap) is a bit of a per-row mask computed once; tap / channel-chunk / stage / phase are running counters (no divisions)
-//  * the per-channel BatchNorm partial sums of a 32 x 32 accumulator block use a transposing reduction (31 shuffles instead of 160)
-//    and are stored as one coalesced 256-byte row per warp
-//  * EPI == 1 (BasicBlock tail): the 1x1 shortcut convolution adds the normalised main branch and applies ReLU in its epilogue,
-//    out = relu(resid * scale + shift + conv(x) + bias) as bf16, which removes the fp32 round trip of the shortcut and one
-//    BN-apply kernel per block (BasicBlock.forward, Modules.py:128-142)
-//  * NPW = 4 or 8 producer warps (GQ_NPW): 8 halves the copies per thread and lets warps 4-7 take half of the epilogue columns (a warp
-//    may read the TMEM lane quarter warp % 4, so warps w and w + 4 share rows and split columns)
-//  * TMAB = 1 (default; GQ_TMA=0 disables): the weight tile of a k-step (two thirds of the bytes at BLOCK_N = 256) is one TMA box issued by one thread
-//    instead of BLOCK_N / RS cp.async per producer thread; the activation gather stays on cp.async (its rows are not a box)
-template <int BLOCK_N, int STAGES, int EPI, int NPW, int TMAB>
-__global__ void __launch_bounds__(32 * (NPW + 1)) k_conv_tc(const __grid_constant__ CUtensorMap tmap_w, const bf16* __restrict__ x,
-                                                            const bf16* __restrict__ w, const float* __restrict__ bias,
-                                                 float* __restrict__ y, float* __restrict__ stats, const float* __restrict__ resid,
-                                                 const float2* __restrict__ scale_shift, bf16* __restrict__ out, int H, int W, int Cin, int Cout,
-                                                 int ks, int cg_weights) {
-  constexpr int A_STAGE = BM * BK * 2, B_STAGE = BLOCK_N * BK * 2;  // bytes
-  extern __shared__ __align__(1024) uint8_t smem[];
-  uint8_t* sA = smem;
-  uint8_t* sB = smem + STAGES * A_STAGE;
-  uint64_t* full = (uint64_t*)(smem + STAGES * (A_STAGE + B_STAGE));  // [STAGES] copies landed (32 NPW producer arrivals)
-  uint64_t* empty = full + STAGES;                                    // [STAGES] MMAs that read the stage are done (1 commit)
-  uint64_t* accbar = empty + STAGES;                                  // accumulator complete
-  uint32_t* tmem_slot = (uint32_t*)(accbar + 1);
-  constexpr int RS = 4 * NPW;  // row step of the copy mapping (qnet_plan.h): producer threads / 8
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int HW = H * W, m0 = blockIdx.x * BM, n0 = blockIdx.y * BLOCK_N, b = blockIdx.z;
-  const int pad = ks / 2, taps = ks * ks, kchunks = Cin / BK, nk = taps * kchunks;
-  if (tid == 0) {
-    for (int i = 0; i < STAGES; i++) { mbar_init(&full[i], 32 * NPW + TMAB); mbar_init(&empty[i], 1); }
-    mbar_init(accbar, 1);
-    fence_barrier_init();
-  }
-  if (warp == 0) tmem_alloc(tmem_slot, BLOCK_N);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tacc = *tmem_slot;
-  constexpr uint32_t idesc = make_idesc(BM, BLOCK_N);
-  if (warp < NPW) {
-    // ---- producers.  Thread -> 16-byte chunk tid % 8 of rows tid / 8 + RS i (consecutive lanes take consecutive chunks of one
-    // row: a warp-level cp.async reads 4 full 128-byte lines and writes 4 swizzled, conflict-free shared-memory rows).  The plan
-    // (qnet_plan.h) holds the per-thread constants and the running tap / chunk / stage counters.
-    ConvPlan p;
-    conv_plan_init<RS>(p, tid, m0, n0, H, W, Cin, ks);
-    const uint32_t sA_u = smem_u32(sA) + p.dstoff, sB_u = smem_u32(sB) + p.dstoff;
-    const char* xb = (const char*)(x + (size_t)b * HW * Cin);
-    const char* wb = (const char*)w;
-    for (int kn = 0; kn < nk; kn++) {
-      if (p.round > 0) mbar_wait(&empty[p.sn], (uint32_t)(p.round - 1) & 1u);  // the MMAs of k-step kn - STAGES have read the stage
-      const uint32_t tbit = 1u << p.tap;
-      const char* ap = xb + conv_plan_a(p, W, Cin);
-      const uint32_t da = sA_u + (uint32_t)(p.sn * A_STAGE);
-#pragma unroll
-      for (int i = 0; i < BM / RS; i++) {
-        const bool ok = (p.vmask[i] & tbit) != 0;
-        cp_async16_s(da + i * (RS * 128), ok ? (const void*)ap : (const void*)xb, ok ? 16u : 0u);
-        ap += p.a_stride;
-      }
-      if constexpr (TMAB) {
-        if (tid == 0) {  // box = rows n0 .. n0 + BLOCK_N - 1, columns 64 kn .. 64 kn + 63 of w viewed as [Cout][taps * Cin]
-          mbar_arrive_expect_tx(&full[p.sn], (uint32_t)B_STAGE);
-          tma_load_2d(smem_u32(sB) + (uint32_t)(p.sn * B_STAGE), &tmap_w, kn * BK, n0, &full[p.sn]);
-        }
-      } else {
-        const char* bp = wb + conv_plan_b(p, kn);
-        const uint32_t db = sB_u + (uint32_t)(p.sn * B_STAGE);
-#pragma unroll
-        for (int i = 0; i < BLOCK_N / RS; i++) {
-          if (cg_weights) cp_async16_cg(db + i * (RS * 128), bp); else cp_async16_s(db + i * (RS * 128), bp, 16u);
-          bp += p.b_stride;
-        }
-      }
-      cp_async_mbar_arrive(&full[p.sn]);
-      conv_plan_next(p, STAGES, kchunks, pad);
-    }
-  } else if (lane == 0) {  // warp NPW: the MMA issuer
-    int s = 0; uint32_t ph = 0;
-    for (int kb = 0; kb < nk; kb++) {
-      mbar_wait(&full[s], ph);
-      fence_proxy_async();  // generic-proxy (cp.async) smem writes -> visible to the tensor core (async proxy)
-      tc_fence_after();
-      const uint32_t a_base = smem_u32(sA + s * A_STAGE), b_base = smem_u32(sB + s * B_STAGE);
-#pragma unroll
-      for (int k = 0; k < BK / 16; k++) {  // UMMA_K = 16 bf16 = 32 bytes inside the swizzle atom
-        uint64_t adesc = make_smem_desc_sw128(a_base + k * 32);
-        uint64_t bdesc = make_smem_desc_sw128(b_base + k * 32);
-        umma_bf16(tacc, adesc, bdesc, idesc, (kb > 0 || k > 0) ? 1u : 0u);
-      }
-      umma_commit(&empty[s]);
-      if (kb == nk - 1) umma_commit(accbar);
-      if (++s == STAGES) { s = 0; ph ^= 1u; }
-    }
-  }
-  if (warp < NPW) {
-    mbar_wait(accbar, 0);
-    tc_fence_after();
-    // ---- epilogue: lane t of a warp with warp % 4 == q holds accumulator row 32 q + t; with 8 warps, warps 4-7 take the upper half of
-    // the columns
-    const int quarter = warp & 3;
-    const int m = m0 + quarter * 32 + lane;
-    const bool mvalid = m < HW;
-    const size_t rowoff = ((size_t)b * HW + m) * Cout + n0;
-    constexpr int CB_PER_WARP = BLOCK_N / (NPW / 4);
-    const int cb0 = (warp >> 2) * CB_PER_WARP;
-    for (int cb = cb0; cb < cb0 + CB_PER_WARP; cb += 32) {
-      float v[32];
-      tmem_ld32(tacc + ((uint32_t)(quarter * 32) << 16) + cb, v);
-      if (bias) {
-        const float4* b4 = (const float4*)(bias + n0 + cb);
-#pragma unroll
-        for (int i = 0; i < 8; i++) { const float4 bv = __ldg(b4 + i); v[4 * i] += bv.x; v[4 * i + 1] += bv.y; v[4 * i + 2] += bv.z; v[4 * i + 3] += bv.w; }
-      }
-      if constexpr (EPI == 0) {
-        if (mvalid) {
-          float4* dst = (float4*)(y + rowoff + cb);
-#pragma unroll
-          for (int i = 0; i < 8; i++) dst[i] = make_float4(v[4 * i], v[4 * i + 1], v[4 * i + 2], v[4 * i + 3]);
-        }
-        if (stats) {
-          float q[32];
-#pragma unroll
-          for (int i = 0; i < 32; i++) { v[i] = mvalid ? v[i] : 0.f; q[i] = v[i] * v[i]; }
-          const float s1 = warp_colsum32(v, lane), s2 = warp_colsum32(q, lane);
-          // deterministic: every (CTA, warp) writes its own partial row, k_bn_reduce adds them in a fixed order
-          float2* pp = (float2*)(stats + ((((size_t)b * gridDim.x + blockIdx.x) * 4 + quarter) * Cout + n0 + cb) * 2);
-          pp[lane] = make_float2(s1, s2);
-        }
-      } else {
-        if (mvalid) {
-          const float4* r4 = (const float4*)(resid + rowoff + cb);
-          const float4* ss4 = (const float4*)(scale_shift + (size_t)b * Cout + n0 + cb);  // (scale, shift) pairs
-          __nv_bfloat162 o[16];
-#pragma unroll
-          for (int i = 0; i < 8; i++) {
-            const float4 r = __ldg(r4 + i);
-            const float4 sa = __ldg(ss4 + 2 * i), sb = __ldg(ss4 + 2 * i + 1);  // columns 4i, 4i+1 | 4i+2, 4i+3
-            const float o0 = fmaxf(r.x * sa.x + sa.y + v[4 * i], 0.f), o1 = fmaxf(r.y * sa.z + sa.w + v[4 * i + 1], 0.f);
-            const float o2 = fmaxf(r.z * sb.x + sb.y + v[4 * i + 2], 0.f), o3 = fmaxf(r.w * sb.z + sb.w + v[4 * i + 3], 0.f);
-            o[2 * i] = __floats2bfloat162_rn(o0, o1); o[2 * i + 1] = __floats2bfloat162_rn(o2, o3);
-          }
-          uint4* dst = (uint4*)(out + rowoff + cb);
-#pragma unroll
-          for (int i = 0; i < 4; i++) dst[i] = ((const uint4*)o)[i];
-        }
-      }
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) tmem_dealloc(tacc, BLOCK_N);
-}
-// epilogue of one 128 x BLOCK_N accumulator (TMEM columns tcol .. tcol + BLOCK_N - 1) for the warp owning lane quarter `quarter`:
-// the same arithmetic as the epilogue of k_conv_tc
-template <int BLOCK_N, int EPI>
-__device__ __forceinline__ void conv_epilogue_tile(uint32_t tcol, int quarter, int lane, int mt, int n0, int b, int gx, int HW, int Cout,
-                                                   const float* __restrict__ bias, float* __restrict__ y, float* __restrict__ stats,
-                                                   const float* __restrict__ resid, const float2* __restrict__ scale_shift, bf16* __restrict__ out) {
-  const int m = mt * BM + quarter * 32 + lane;
-  const bool mvalid = m < HW;
-  const size_t rowoff = ((size_t)b * HW + m) * Cout + n0;
-  for (int cb = 0; cb < BLOCK_N; cb += 32) {
-    float v[32];
-    tmem_ld32(tcol + ((uint32_t)(quarter * 32) << 16) + (uint32_t)cb, v);
-    if (bias) {
-      const float4* b4 = (const float4*)(bias + n0 + cb);
-#pragma unroll
-      for (int j = 0; j < 8; j++) { const float4 bv = __ldg(b4 + j); v[4 * j] += bv.x; v[4 * j + 1] += bv.y; v[4 * j + 2] += bv.z; v[4 * j + 3] += bv.w; }
-    }
-    if constexpr (EPI == 0) {
-      if (mvalid) {
-        float4* dst = (float4*)(y + rowoff + cb);
-#pragma unroll
-        for (int j = 0; j < 8; j++) dst[j] = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-      }
-      if (stats) {
-        float q[32];
-#pragma unroll
-        for (int j = 0; j < 32; j++) { v[j] = mvalid ? v[j] : 0.f; q[j] = v[j] * v[j]; }
-        const float s1 = warp_colsum32(v, lane), s2 = warp_colsum32(q, lane);
-        float2* pp = (float2*)(stats + ((((size_t)b * gx + mt) * 4 + quarter) * Cout + n0 + cb) * 2);
-        pp[lane] = make_float2(s1, s2);
-      }
-    } else {
-      if (mvalid) {
-        const float4* r4 = (const float4*)(resid + rowoff + cb);
-        const float4* ss4 = (const float4*)(scale_shift + (size_t)b * Cout + n0 + cb);
-        __nv_bfloat162 o[16];
-#pragma unroll
-        for (int j = 0; j < 8; j++) {
-          const float4 r = __ldg(r4 + j);
-          const float4 sa = __ldg(ss4 + 2 * j), sb = __ldg(ss4 + 2 * j + 1);
-          const float o0 = fmaxf(r.x * sa.x + sa.y + v[4 * j], 0.f), o1 = fmaxf(r.y * sa.z + sa.w + v[4 * j + 1], 0.f);
-          const float o2 = fmaxf(r.z * sb.x + sb.y + v[4 * j + 2], 0.f), o3 = fmaxf(r.w * sb.z + sb.w + v[4 * j + 3], 0.f);
-          o[2 * j] = __floats2bfloat162_rn(o0, o1); o[2 * j + 1] = __floats2bfloat162_rn(o2, o3);
-        }
-        uint4* dst = (uint4*)(out + rowoff + cb);
-#pragma unroll
-        for (int j = 0; j < 4; j++) dst[j] = ((const uint4*)o)[j];
-      }
-    }
-  }
-}
-
-// ---- DEFAULT since r02a: the persistent kernel fed by TMA only (whole forward 477 vs 439 TFLOP/s, profiles/r02a_qnet_sweep.txt; a
-// second persistent variant with a cp.async activation gather measured 409 and was deleted).  One CTA per SM walks a static
-// round-robin list of (m tile, n tile, image) tiles; the accumulator is double-buffered in TMEM (2 x BLOCK_N columns) and the epilogue
-// has its own 4 warps, so the TMEM read-out, the stores and the BatchNorm partials of tile i overlap the main loop of tile i + 1.  The
-// activation operand is an **im2col-mode** tensor map over x [N][H][W][C] (cuTensorMapEncodeIm2col: pixel box corners (-pad, -pad) /
-// (pad - (ks - 1), ...), 64 channels per pixel, 128 pixels per column, 128-byte swizzle): one
-// `cp.async.bulk.tensor.4d...im2col` per k-step loads the 128 consecutive output positions of the tile for filter tap (offset_w, offset_h)
-// with hardware zero fill at the image border - the same [128 pixels x 64 channels] swizzled tile the cp.async gather builds (semantics
-// as used by CUTLASS' sm100 implicit-GEMM collective: start coordinate = first output pixel + lower corner, tap passed as offsets).
-// One thread issues both TMAs of a k-step after a single arrive.expect_tx(A + B bytes) on the stage's full barrier (count 1).
-// Roles: warp 0 lane 0 producer, warp 1 lane 0 MMA issuer, warps 2-5 epilogue (lane quarter warp % 4).
+// im2col mode: the 128 consecutive output positions starting at pixel (w, h) of image n, for filter tap (off_w, off_h), 64 channels from c;
+// hardware zero fill outside the image (the convolution padding)
 __device__ __forceinline__ void tma_load_im2col_4d(uint32_t dst_smem_addr, const CUtensorMap* tmap, int c, int w, int h, int n, uint16_t off_w,
                                                    uint16_t off_h, uint64_t* bar) {
   asm volatile("cp.async.bulk.tensor.4d.shared::cluster.global.im2col.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2], {%7, %8};"
                ::"r"(dst_smem_addr), "l"((uint64_t)tmap), "r"(smem_u32(bar)), "r"(c), "r"(w), "r"(h), "r"(n), "h"(off_w), "h"(off_h) : "memory");
 }
+
+// ---- wgmma (sm_90a).  A and B both from shared memory; TA / TB = 1 marks an MN-major operand (the weight gradient), 0 a K-major one.
+// Shared-memory matrix descriptor, SWIZZLE_128B: start address, leading byte offset (MN-major: distance of the next 64-element block
+// along M / N; unused for K-major), stride byte offset (distance of the next 8-row group: 8 x 128 B), layout type 1 = 128-byte swizzle.
+__device__ __forceinline__ uint64_t gmma_desc_sw128(uint32_t saddr, uint32_t lbo_bytes) {
+  uint64_t d = 0;
+  d |= (uint64_t)((saddr >> 4) & 0x3fff);
+  d |= (uint64_t)((lbo_bytes >> 4) & 0x3fff) << 16;
+  d |= (uint64_t)(1024 >> 4) << 32;
+  d |= (uint64_t)1 << 62;
+  return d;
+}
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n64(float (&d)[32], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, %35, %36;\n\t}"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+               : "l"(adesc), "l"(bdesc), "r"(accumulate), "n"(TA), "n"(TB));
+}
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n128(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, %67, %68;\n\t}"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+               : "l"(adesc), "l"(bdesc), "r"(accumulate), "n"(TA), "n"(TB));
+}
+// D (+)= A * B for one warpgroup: 64 rows x BLOCK_N columns, K = 16
+template <int BLOCK_N, int TA, int TB>
+__device__ __forceinline__ void wgmma_tile(float (&d)[BLOCK_N / 2], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  if constexpr (BLOCK_N == 128) wgmma_m64n128<TA, TB>(d, adesc, bdesc, accumulate);
+  else wgmma_m64n64<TA, TB>(d, adesc, bdesc, accumulate);
+}
+
+// ------------------------------------------------------------------------------------------------ implicit-GEMM convolution on wgmma
+// x  [B,H,W,Cin] bf16 (NHWC), w [Cout][ks*ks][Cin] bf16, y [B,H,W,Cout] f32 (+ bias), partials [B][gx][8][Cout][2] f32 (sum, sum of squares)
+// One tile = 128 output pixels (BM) x BLOCK_N output channels of one image, walked in k-steps of 64 input channels of one filter tap.
+// Persistent: CTA i takes tiles i, i + gridDim.x, ... (m tile fastest, then n tile, then image).  288 threads: warpgroups 0 and 1
+// consume (rows 0-63 / 64-127 of the tile), warp 8 lane 0 produces.  One k-step = one arrive.expect_tx(A + B bytes) on the stage's
+// full barrier (count 1) and two TMAs: the im2col box of the activations (128 output positions x 64 channels for the tap, zero fill
+// at the image border) and the [BLOCK_N x 64] box of the weights, both 128-byte swizzled K-major.  A consumer warpgroup issues the
+// four k16 wgmmas of a stage, keeps one group in flight and releases the previous stage (empty barrier, one arrival per consumer warp,
+// count 8) once wgmma.wait_group 1 says its reads are done.  The producer runs ahead across tile boundaries, so the loads of the next
+// tile overlap the epilogue of the current one.
+#define BM 128
+#define BK 64
+#define CONV_THREADS 288
+#define CONV_PARTS 8  // BatchNorm partial rows per tile: one per consumer warp (gq_conv_partials_floats)
+// epilogue of one warpgroup's 64 x BLOCK_N accumulator (wgmma fragment: row 16 warp + lane / 4 (+ 8), columns 8 j + 2 (lane % 4) + {0, 1})
+//   EPI 0: y = conv + bias (fp32) and, if requested, per-(tile, warp) BatchNorm partials over the warp's 16 rows, reduced over the
+//          lanes in a fixed order (deterministic) and summed in a fixed order by k_bn_reduce
+//   EPI 1 (BasicBlock tail): out = relu(resid * scale + shift + conv + bias) as bf16 (BasicBlock.forward, Modules.py:128-142)
+template <int BLOCK_N, int EPI>
+__device__ __forceinline__ void conv_epilogue(const float (&acc)[BLOCK_N / 2], int wg, int warp, int lane, int mt, int n0, int b, int gx, int HW, int Cout,
+                                              const float* __restrict__ bias, float* __restrict__ y, float* __restrict__ stats,
+                                              const float* __restrict__ resid, const float2* __restrict__ scale_shift, bf16* __restrict__ out) {
+  const int wq = warp & 3;
+  const int ma = mt * BM + wg * 64 + wq * 16 + (lane >> 2), mb = ma + 8;
+  const bool va = ma < HW, vb = mb < HW;
+  const size_t rowa = ((size_t)b * HW + ma) * Cout, rowb = ((size_t)b * HW + mb) * Cout;
+#pragma unroll
+  for (int j = 0; j < BLOCK_N / 8; j++) {
+    const int c = n0 + 8 * j + 2 * (lane & 3);
+    float x0 = acc[4 * j], x1 = acc[4 * j + 1], x2 = acc[4 * j + 2], x3 = acc[4 * j + 3];
+    if (bias) { const float2 bv = __ldg((const float2*)(bias + c)); x0 += bv.x; x1 += bv.y; x2 += bv.x; x3 += bv.y; }
+    if constexpr (EPI == 0) {
+      if (va) *(float2*)(y + rowa + c) = make_float2(x0, x1);
+      if (vb) *(float2*)(y + rowb + c) = make_float2(x2, x3);
+      if (stats) {
+        if (!va) { x0 = 0.f; x1 = 0.f; }
+        if (!vb) { x2 = 0.f; x3 = 0.f; }
+        float s0 = x0 + x2, s1 = x1 + x3, q0 = x0 * x0 + x2 * x2, q1 = x1 * x1 + x3 * x3;
+#pragma unroll
+        for (int o = 4; o < 32; o <<= 1) {
+          s0 += __shfl_xor_sync(0xffffffffu, s0, o); s1 += __shfl_xor_sync(0xffffffffu, s1, o);
+          q0 += __shfl_xor_sync(0xffffffffu, q0, o); q1 += __shfl_xor_sync(0xffffffffu, q1, o);
+        }
+        if (lane < 4) *(float4*)(stats + ((((size_t)b * gx + mt) * CONV_PARTS + wg * 4 + wq) * Cout + c) * 2) = make_float4(s0, q0, s1, q1);
+      }
+    } else {
+      const float4 ss = __ldg((const float4*)(scale_shift + (size_t)b * Cout + c));  // (scale, shift) of columns c, c + 1
+      if (va) {
+        const float2 r = __ldg((const float2*)(resid + rowa + c));
+        *(__nv_bfloat162*)(out + rowa + c) = __floats2bfloat162_rn(fmaxf(r.x * ss.x + ss.y + x0, 0.f), fmaxf(r.y * ss.z + ss.w + x1, 0.f));
+      }
+      if (vb) {
+        const float2 r = __ldg((const float2*)(resid + rowb + c));
+        *(__nv_bfloat162*)(out + rowb + c) = __floats2bfloat162_rn(fmaxf(r.x * ss.x + ss.y + x2, 0.f), fmaxf(r.y * ss.z + ss.w + x3, 0.f));
+      }
+    }
+  }
+}
 template <int BLOCK_N, int STAGES, int EPI>
-__global__ void __launch_bounds__(192) k_conv_tc_tma(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant__ CUtensorMap tmap_x,
-                                                     const float* __restrict__ bias, float* __restrict__ y, float* __restrict__ stats,
-                                                     const float* __restrict__ resid, const float2* __restrict__ scale_shift, bf16* __restrict__ out,
-                                                     int H, int W, int Cin, int Cout, int ks, int gx, int gy, int ntiles) {
+__global__ void __launch_bounds__(CONV_THREADS, 1) k_conv_wgmma(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant__ CUtensorMap tmap_x,
+                                                               const float* __restrict__ bias, float* __restrict__ y, float* __restrict__ stats,
+                                                               const float* __restrict__ resid, const float2* __restrict__ scale_shift, bf16* __restrict__ out,
+                                                               int H, int W, int Cin, int Cout, int ks, int gx, int gy, int ntiles) {
   constexpr int A_STAGE = BM * BK * 2, B_STAGE = BLOCK_N * BK * 2;
-  extern __shared__ __align__(1024) uint8_t smem[];
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);  // the 128-byte swizzle pattern repeats every 1024 bytes
   uint8_t* sA = smem;
   uint8_t* sB = smem + STAGES * A_STAGE;
   uint64_t* full = (uint64_t*)(smem + STAGES * (A_STAGE + B_STAGE));
   uint64_t* empty = full + STAGES;
-  uint64_t* acc_full = empty + STAGES;
-  uint64_t* acc_empty = acc_full + 2;
-  uint32_t* tmem_slot = (uint32_t*)(acc_empty + 2);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int HW = H * W, pad = ks / 2, taps = ks * ks, kchunks = Cin / BK, nk = taps * kchunks;
+  const int HW = H * W, pad = ks / 2, kchunks = Cin / BK, nk = ks * ks * kchunks;
   if (tid == 0) {
-    for (int i = 0; i < STAGES; i++) { mbar_init(&full[i], 1); mbar_init(&empty[i], 1); }
-    for (int i = 0; i < 2; i++) { mbar_init(&acc_full[i], 1); mbar_init(&acc_empty[i], 128); }
+    for (int i = 0; i < STAGES; i++) { mbar_init(&full[i], 1); mbar_init(&empty[i], 8); }
     fence_barrier_init();
   }
-  if (warp == 0) tmem_alloc(tmem_slot, 2 * BLOCK_N);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tacc = *tmem_slot;
-  constexpr uint32_t idesc = make_idesc(BM, BLOCK_N);
-  if (warp == 0) {
+  if (warp == 8) {
     if (lane == 0) {
       int sn = 0, round = 0;
       for (int t = blockIdx.x; t < ntiles; t += gridDim.x) {
@@ -417,43 +187,35 @@ __global__ void __launch_bounds__(192) k_conv_tc_tma(const __grid_constant__ CUt
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      int s = 0; uint32_t ph = 0; int i = 0;
-      for (int t = blockIdx.x; t < ntiles; t += gridDim.x, i++) {
-        const int a = i & 1;
-        mbar_wait(&acc_empty[a], (uint32_t)((i >> 1) & 1) ^ 1u);
-        tc_fence_after();
-        const uint32_t dacc = tacc + (uint32_t)(a * BLOCK_N);
-        for (int kb = 0; kb < nk; kb++) {
-          mbar_wait(&full[s], ph);  // both operands arrive through the async proxy (TMA): no generic-proxy fence needed
-          tc_fence_after();
-          const uint32_t a_base = smem_u32(sA + s * A_STAGE), b_base = smem_u32(sB + s * B_STAGE);
-#pragma unroll
-          for (int k = 0; k < BK / 16; k++)
-            umma_bf16(dacc, make_smem_desc_sw128(a_base + k * 32), make_smem_desc_sw128(b_base + k * 32), idesc, (kb > 0 || k > 0) ? 1u : 0u);
-          umma_commit(&empty[s]);
-          if (kb == nk - 1) umma_commit(&acc_full[a]);
-          if (++s == STAGES) { s = 0; ph ^= 1u; }
-        }
-      }
-    }
-  } else {
-    const int quarter = warp & 3;
-    int i = 0;
-    for (int t = blockIdx.x; t < ntiles; t += gridDim.x, i++) {
-      const int mt = t % gx, nt = (t / gx) % gy, b = t / (gx * gy);
-      const int a = i & 1;
-      mbar_wait(&acc_full[a], (uint32_t)(i >> 1) & 1u);
-      tc_fence_after();
-      conv_epilogue_tile<BLOCK_N, EPI>(tacc + (uint32_t)(a * BLOCK_N), quarter, lane, mt, nt * BLOCK_N, b, gx, HW, Cout, bias, y, stats, resid, scale_shift, out);
-      tc_fence_before();
-      asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(&acc_empty[a])) : "memory");
-    }
+    return;
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) tmem_dealloc(tacc, 2 * BLOCK_N);
+  const int wg = warp >> 2;
+  int s = 0;
+  uint32_t ph = 0;
+  for (int t = blockIdx.x; t < ntiles; t += gridDim.x) {
+    const int mt = t % gx, nt = (t / gx) % gy, b = t / (gx * gy);
+    float acc[BLOCK_N / 2];
+#pragma unroll
+    for (int i = 0; i < BLOCK_N / 2; i++) acc[i] = 0.f;
+    int prev = -1;
+    for (int kb = 0; kb < nk; kb++) {
+      mbar_wait(&full[s], ph);
+      const uint32_t a_base = smem_u32(sA + s * A_STAGE) + (uint32_t)(wg * 64 * 128), b_base = smem_u32(sB + s * B_STAGE);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < BK / 16; k++)  // K = 16 bf16 = 32 bytes further inside the swizzle atom
+        wgmma_tile<BLOCK_N, 0, 0>(acc, gmma_desc_sw128(a_base + k * 32, 16), gmma_desc_sw128(b_base + k * 32, 16), (kb > 0 || k > 0) ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<1>();  // the wgmmas of the previous stage have completed: release it
+      if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(&empty[prev]); }
+      prev = s;
+      if (++s == STAGES) { s = 0; ph ^= 1u; }
+    }
+    wgmma_wait<0>();
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty[prev]);
+    conv_epilogue<BLOCK_N, EPI>(acc, wg, warp, lane, mt, nt * BLOCK_N, b, gx, HW, Cout, bias, y, stats, resid, scale_shift, out);
+  }
 }
 
 // per-image BatchNorm (training mode, own statistics) folded into one multiply-add per channel: (scale, shift) from (sum, sum of squares)
@@ -468,13 +230,13 @@ __global__ void k_bn_scale_shift(const float* __restrict__ stats, const float* _
   ss[i] = make_float2(scale, beta[c] - mean * scale);
 }
 
-// per-image batch-norm statistics from the per-(tile, warp) partials of k_conv_tc, summed in a fixed order (double accumulation)
+// per-image batch-norm statistics from the per-(tile, warp) partials of k_conv_wgmma, summed in a fixed order (double accumulation)
 __global__ void k_bn_reduce(const float* __restrict__ part, float* __restrict__ stats, int B, int nparts, int C) {
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= B * C) return;
   int b = i / C, c = i % C;
   // one accumulator pair in part order (the order is part of the result); the unrolled body keeps 8 independent 8-byte loads in flight
-  // (r01j: a 4-accumulator version with a dynamically indexed remainder went to local memory and ran 2.7x slower - reverted)
+  // (a 4-accumulator version with a dynamically indexed remainder goes to local memory)
   double s1 = 0, s2 = 0;
   const float2* p = (const float2*)part + (size_t)b * nparts * C + c;
 #pragma unroll 8
@@ -869,30 +631,17 @@ extern "C" int gq_obs_to_state(const unsigned char* rgb, const float* depth, flo
   QCK(cudaGetLastError());
   return 0;
 }
-extern "C" const char* gq_version(void) { return "grasp_qnet 0.5 sm_100a bf16 tcgen05 (persistent CTAs, both operands by TMA: im2col activations + tiled weights, SW128 K-major, double-buffered TMEM accumulator, fused block tail)"; }
 
-// tile shape: 128 output pixels x 64 / 128 / 256 output channels (the widest that divides Cout).  Tuning overrides: GQ_BN=128,
-// GQ_PERSIST=0 (non-persistent kernel: 3 stages, GQ_NPW=4|8 producer warps, GQ_CGB=1 weights bypass L1, GQ_TMA=0 weight tiles by cp.async).
-struct ConvCfg { int bn, npw, cg, tma, persist; };
-static ConvCfg conv_cfg(int Cout) {
-  static int env_bn = -1, env_npw = 8, env_cg = 0, env_tma = 1, env_persist = 2;
-  if (env_bn < 0) {
-    const char* e = getenv("GQ_BN"); env_bn = e ? atoi(e) : 0;
-    e = getenv("GQ_NPW"); env_npw = (e && atoi(e) == 4) ? 4 : 8;  // r01i sweep, whole forward: 4 warps 366, 8 warps 381 TFLOP/s
-    e = getenv("GQ_CGB"); env_cg = (e && atoi(e) != 0) ? 1 : 0;
-    e = getenv("GQ_PERSIST"); env_persist = (e && atoi(e) == 0) ? 0 : 2;  // r02a: persistent TMA kernel 477, non-persistent 439 TFLOP/s
-    e = getenv("GQ_TMA"); env_tma = (e && atoi(e) == 0) ? 0 : 1;  // r01k: weight tiles by TMA 439 vs 414 TFLOP/s whole forward
-  }
-  ConvCfg c;
-  c.bn = (Cout % 128 == 0) ? 128 : 64;
-  if (env_bn != 128 && Cout % 256 == 0) c.bn = 256;
-  c.npw = env_npw; c.cg = env_cg; c.tma = env_tma; c.persist = env_persist;
-  return c;
-}
-static size_t conv_smem(int bn, int nst) { return (size_t)nst * (BM * BK * 2) + (size_t)nst * ((size_t)bn * BK * 2) + 8 * (2 * nst + 1) + 16; }
+extern "C" const char* gq_version(void) { return "grasp_qnet 0.6 sm_90a bf16 wgmma (persistent CTAs, both operands by TMA: im2col activations + tiled weights, SW128 K-major, register accumulators, fused block tail)"; }
+
+// tile shape: 128 output pixels x 128 output channels (64 when 128 does not divide Cout); the accumulator of a consumer warpgroup is
+// 64 x BLOCK_N fp32 = BLOCK_N / 2 registers per thread.  One CTA per SM with 192 KB of stages (6 at BLOCK_N 128, 8 at 64): on an H100
+// (700 W) the whole forward ran at 297 TFLOP/s this way against 287 with two CTAs per SM of 96 KB each, whose 96-register cap spilled.
+static int conv_block_n(int Cout) { return (Cout % 128 == 0) ? 128 : 64; }
+static size_t conv_smem(int bn, int nst) { return 1024 + (size_t)nst * (BM * BK * 2 + (size_t)bn * BK * 2) + 16 * (size_t)nst; }
 
 // 2-D tensor map of the packed weights w [Cout][taps * Cin] bf16 with a [BLOCK_N rows x 64 columns] box, 128-byte swizzle (the layout the
-// UMMA descriptors expect); cuTensorMapEncodeTiled comes from the driver through the runtime (no libcuda link dependency)
+// wgmma descriptors expect); cuTensorMapEncodeTiled comes from the driver through the runtime (no libcuda link dependency)
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
                                   const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 static int make_weight_tmap(CUtensorMap* m, const void* w, int Cout, int K, int bn) {
@@ -940,74 +689,46 @@ static int make_act_tmap_im2col(CUtensorMap* m, const void* x, int B, int H, int
   return 0;
 }
 
-// EPI 0: y (+ BN partials); EPI 1: out = relu(resid * scale + shift + conv + bias) bf16
+// EPI 0: y (+ BN partials); EPI 1: out = relu(resid * scale + shift + conv + bias) bf16.  grid = (m tiles, n tiles, images) of the problem.
 template <int EPI>
-static int launch_conv(const ConvCfg& c, dim3 grid, cudaStream_t st, const bf16* x, const bf16* w, const float* bias, float* y, float* partials,
+static int launch_conv(int bn, dim3 grid, cudaStream_t st, const bf16* x, const bf16* w, const float* bias, float* y, float* partials,
                        const float* resid, const float2* ss, bf16* out, int H, int W, int Cin, int Cout, int ks) {
-  const size_t smem = conv_smem(c.bn, 3);
-  alignas(64) CUtensorMap tm;
+  alignas(64) CUtensorMap tm, tmx;
   memset(&tm, 0, sizeof tm);
-  bool tma = c.tma != 0;
-  if (tma && make_weight_tmap(&tm, w, Cout, ks * ks * Cin, c.bn) != 0) {  // no encoder in this driver: same kernel with cp.async weight copies
-    static bool told = false;
-    if (!told) { told = true; fprintf(stderr, "grasp_qnet: %s; weight tiles fall back to cp.async\n", q_err); }
-    tma = false;
-  }
-  if (c.persist && tma) {
-    // one CTA per SM, static tile list, 192 KB of stages (4 / 6 / 8 at BLOCK_N 256 / 128 / 64)
-    int dev = 0, sms = 148;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    const int gx = (int)grid.x, gy = (int)grid.y, ntiles = gx * gy * (int)grid.z;
-    const int nctas = ntiles < sms ? ntiles : sms;
-    alignas(64) CUtensorMap tmx;
-    static bool im2col_ok = true;
-    if (im2col_ok && make_act_tmap_im2col(&tmx, x, (int)grid.z, H, W, Cin, ks) != 0) {
-      im2col_ok = false;
-      fprintf(stderr, "grasp_qnet: %s; using the non-persistent kernel\n", q_err);
-    }
-    if (im2col_ok) {
-#define LAUNCH_T(BN_, ST_)                                                                                                           \
-  do {                                                                                                                               \
-    const size_t psmem = (size_t)ST_ * (BM * BK * 2 + BN_ * BK * 2) + 8 * (2 * ST_ + 4) + 16;                                         \
-    QCK(cudaFuncSetAttribute(k_conv_tc_tma<BN_, ST_, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)psmem));                 \
-    k_conv_tc_tma<BN_, ST_, EPI><<<nctas, 192, psmem, st>>>(tm, tmx, bias, y, partials, resid, ss, out, H, W, Cin, Cout, ks, gx, gy, ntiles); \
+  memset(&tmx, 0, sizeof tmx);
+  int r = make_weight_tmap(&tm, w, Cout, ks * ks * Cin, bn);
+  if (r == 0) r = make_act_tmap_im2col(&tmx, x, (int)grid.z, H, W, Cin, ks);
+  if (r) return r;
+  int dev = 0, sms = 0;
+  QCK(cudaGetDevice(&dev));
+  QCK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  const int gx = (int)grid.x, gy = (int)grid.y, ntiles = gx * gy * (int)grid.z;
+  const int nctas = ntiles < sms ? ntiles : sms;
+#define LAUNCH_T(BN_, ST_)                                                                                                             \
+  do {                                                                                                                                 \
+    const size_t smem = conv_smem(BN_, ST_);                                                                                           \
+    QCK(cudaFuncSetAttribute(k_conv_wgmma<BN_, ST_, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));                     \
+    k_conv_wgmma<BN_, ST_, EPI><<<nctas, CONV_THREADS, smem, st>>>(tm, tmx, bias, y, partials, resid, ss, out, H, W, Cin, Cout, ks, gx, gy, ntiles); \
   } while (0)
-      if (c.bn == 256) LAUNCH_T(256, 4);
-      else if (c.bn == 128) LAUNCH_T(128, 6);
-      else LAUNCH_T(64, 8);
+  if (bn == 128) LAUNCH_T(128, 6);
+  else LAUNCH_T(64, 8);
 #undef LAUNCH_T
-      return 0;
-    }
-  }
-#define LAUNCH_ONE(BN_, NPW_, TMA_)                                                                                                  \
-  do {                                                                                                                               \
-    QCK(cudaFuncSetAttribute(k_conv_tc<BN_, 3, EPI, NPW_, TMA_>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));            \
-    k_conv_tc<BN_, 3, EPI, NPW_, TMA_><<<grid, 32 * (NPW_ + 1), smem, st>>>(tm, x, w, bias, y, partials, resid, ss, out, H, W, Cin, Cout, ks, c.cg); \
-  } while (0)
-#define LAUNCH_CONV(BN_)                                                                                                             \
-  do {                                                                                                                               \
-    if (c.npw == 8) { if (tma) LAUNCH_ONE(BN_, 8, 1); else LAUNCH_ONE(BN_, 8, 0); }                                                  \
-    else { if (tma) LAUNCH_ONE(BN_, 4, 1); else LAUNCH_ONE(BN_, 4, 0); }                                                             \
-  } while (0)
-  if (c.bn == 256) LAUNCH_CONV(256);
-  else if (c.bn == 128) LAUNCH_CONV(128);
-  else LAUNCH_CONV(64);
-#undef LAUNCH_CONV
-#undef LAUNCH_ONE
   return 0;
 }
 
+extern "C" size_t gq_conv_partials_floats(int B, int H, int W, int Cout) {
+  return (size_t)B * ((H * W + BM - 1) / BM) * CONV_PARTS * Cout * 2;
+}
 extern "C" int gq_conv_tc(const void* x, const void* w, const float* bias, float* y, float* stats, float* partials, int B, int H, int W, int Cin, int Cout, int ks,
                           void* stream) {
   if (!x || !w || !y || (ks != 1 && ks != 3) || Cin % 64 || Cout % 64) { snprintf(q_err, sizeof q_err, "gq_conv_tc: bad argument"); return -1; }
   if (stats && !partials) { snprintf(q_err, sizeof q_err, "gq_conv_tc: stats requested without a partials buffer"); return -1; }
   cudaStream_t st = (cudaStream_t)stream;
-  const ConvCfg c = conv_cfg(Cout);
-  dim3 grid((H * W + BM - 1) / BM, Cout / c.bn, B);
-  int r = launch_conv<0>(c, grid, st, (const bf16*)x, (const bf16*)w, bias, y, stats ? partials : nullptr, nullptr, nullptr, nullptr, H, W, Cin, Cout, ks);
+  const int bn = conv_block_n(Cout);
+  dim3 grid((H * W + BM - 1) / BM, Cout / bn, B);
+  int r = launch_conv<0>(bn, grid, st, (const bf16*)x, (const bf16*)w, bias, y, stats ? partials : nullptr, nullptr, nullptr, nullptr, H, W, Cin, Cout, ks);
   if (r) return r;
-  if (stats) k_bn_reduce<<<(B * Cout + 127) / 128, 128, 0, st>>>(partials, stats, B, (int)grid.x * 4, Cout);
+  if (stats) k_bn_reduce<<<(B * Cout + 127) / 128, 128, 0, st>>>(partials, stats, B, (int)grid.x * CONV_PARTS, Cout);
   QCK(cudaGetLastError());
   return 0;
 }
@@ -1019,10 +740,10 @@ extern "C" int gq_conv_tc_block_out(const void* x, const void* w, const float* b
     return -1;
   }
   cudaStream_t st = (cudaStream_t)stream;
-  const ConvCfg c = conv_cfg(Cout);
-  dim3 grid((H * W + BM - 1) / BM, Cout / c.bn, B);
+  const int bn = conv_block_n(Cout);
+  dim3 grid((H * W + BM - 1) / BM, Cout / bn, B);
   k_bn_scale_shift<<<(B * Cout + 127) / 128, 128, 0, st>>>(stats, gamma, beta, (float2*)scratch_scale_shift, B, Cout, H * W, eps);
-  int r = launch_conv<1>(c, grid, st, (const bf16*)x, (const bf16*)w, bias, nullptr, nullptr, resid, (const float2*)scratch_scale_shift, (bf16*)out, H, W, Cin, Cout, ks);
+  int r = launch_conv<1>(bn, grid, st, (const bf16*)x, (const bf16*)w, bias, nullptr, nullptr, resid, (const float2*)scratch_scale_shift, (bf16*)out, H, W, Cin, Cout, ks);
   if (r) return r;
   QCK(cudaGetLastError());
   return 0;
@@ -1044,8 +765,11 @@ extern "C" int gq_maxpool(const void* x, void* y, int B, int H, int W, int C, vo
 extern "C" int gq_bn_act(const float* x, const float* stats, const float* gamma, const float* beta, const float* identity, void* y, int B, int HW, int C,
                          float eps, void* stream) {
   if (C % 8) { snprintf(q_err, sizeof q_err, "gq_bn_act: C must be a multiple of 8"); return -1; }
-  // enough CTAs per image to fill the GPU (148 SMs x 8) without making the per-CTA prologue (2 C floats) matter
-  int ctas = (148 * 8 + B - 1) / B;
+  // enough CTAs per image to fill the GPU (8 per SM) without making the per-CTA prologue (2 C floats) matter
+  int dev = 0, sms = 0;
+  QCK(cudaGetDevice(&dev));
+  QCK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  int ctas = (sms * 8 + B - 1) / B;
   int ppc = (HW + ctas - 1) / ctas;
   if (ppc < 16) ppc = 16;
   dim3 grid((HW + ppc - 1) / ppc, B);

@@ -10,9 +10,9 @@
 //
 // Data layout as in the forward: activations NHWC bf16, pre-BatchNorm convolution outputs fp32, weights [Cout][kh][kw][Cin].
 // Gradients of activations travel as bf16 between layers (fp32 inside a kernel), weight gradients and the optimiser state are fp32.
-//   dgrad (gradient w.r.t. the convolution input) = the forward tcgen05 convolution applied to dY with the spatially flipped,
+//   dgrad (gradient w.r.t. the convolution input) = the forward wgmma convolution applied to dY with the spatially flipped,
 //          in/out-transposed weights (gq_conv_tc called by the host wrapper);
-//   wgrad (gradient w.r.t. the weights)           = k_wgrad_tc below: tcgen05 GEMM with K = pixels, both operands MN-major straight from the
+//   wgrad (gradient w.r.t. the weights)           = k_wgrad_wgmma below: wgmma GEMM with K = pixels, both operands MN-major straight from the
 //          NHWC tensors by TMA (k_wgrad, a CUDA-core tiled kernel, is its A/B partner), split-K over the images of the batch (partials
 //          reduced in image order: deterministic);
 //   everything else is element-wise / reduction glue.
@@ -99,8 +99,8 @@ __global__ void __launch_bounds__(256) k_bn_bwd_reduce(const bf16* __restrict__ 
                                                        const float* __restrict__ stats, int rows, int C, int HW, float eps, int rows_per_cta,
                                                        bf16* __restrict__ dpre_out, float* __restrict__ part) {
   // 256 threads = Cw channels x RL row lanes (Cw = min(C, 256)): consecutive threads read consecutive channels of a row (coalesced), row lane
-  // rl takes rows r0 + rl, r0 + rl + RL, ...; the row lanes are added in fixed order through shared memory.  (r02k: with one thread per
-  // channel only 64 / 128 of the 256 threads worked in the 64- / 128-channel layers.)
+  // rl takes rows r0 + rl, r0 + rl + RL, ...; the row lanes are added in fixed order through shared memory.  (With one thread per
+  // channel only 64 / 128 of the 256 threads would work in the 64- / 128-channel layers.)
   __shared__ float sh[2][256];
   const int r0 = blockIdx.x * rows_per_cta, r1 = min(rows, r0 + rows_per_cta);
   for (int cb = 0; cb < C; cb += 256) {
@@ -129,8 +129,8 @@ __global__ void __launch_bounds__(256) k_bn_bwd_reduce(const bf16* __restrict__ 
   }
 }
 // sums[C,2] = per-channel totals of the partials; dgamma[c] = sums[c][1], dbeta[c] = sums[c][0].  One warp per channel: lane l adds parts
-// l, l + 32, ... in order, then a fixed butterfly over the lanes (deterministic; r02k: one THREAD per channel walked ~1000 partials and
-// the 24 launches took 0.8 ms of a 9 ms update).
+// l, l + 32, ... in order, then a fixed butterfly over the lanes (deterministic; one thread per channel would walk ~1000 partials
+// alone).
 __global__ void __launch_bounds__(128) k_bn_bwd_sums(const float* __restrict__ part, int nparts, int C, float* __restrict__ sums, float* __restrict__ dgamma, float* __restrict__ dbeta) {
   const int c = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
   if (c >= C) return;
@@ -262,8 +262,7 @@ __global__ void __launch_bounds__(256) k_wgrad(const bf16* __restrict__ dY, cons
 // first convolution (4 -> 64 channels, 3x3, no bias; Modules.py:163): dW[co][tap][c] = sum_{b,p} dY[b,p,co] * x[b,c,p+tap] with x the
 // network input [B,4,H,W] f32.  One CTA = one chunk of pixels for ALL 36 (tap, c) pairs: thread (co, quarter) walks a quarter of the
 // chunk with 36 accumulators (dY read once; the 36 input values of a pixel are the same for all threads = broadcast loads), the four
-// quarters are added in fixed order -> part [chunks][64][36].  (r02h: the first version - one CTA of 64 threads per (tap, c, chunk),
-// dY read 36 times - took 3.5 ms of a 28.8 ms update.)
+// quarters are added in fixed order -> part [chunks][64][36].  (One CTA of 64 threads per (tap, c, chunk) would read dY 36 times.)
 __global__ void __launch_bounds__(256) k_conv_first_wgrad(const bf16* __restrict__ dY, const float* __restrict__ x, float* __restrict__ part, int B, int H, int W,
                                                           int pix_per_cta) {
   __shared__ float red[4][64][37];
@@ -323,7 +322,6 @@ __global__ void k_maxpool_bwd(const bf16* __restrict__ x, const bf16* __restrict
   dX[i] = __float2bfloat16(g);
 }
 // the same, 8 channels per thread (16-byte loads; C % 8 == 0): identical arithmetic and window order, an eighth of the load instructions
-// (r02h: the scalar kernel took 1.5 ms of an update for the two pools)
 __global__ void __launch_bounds__(256) k_maxpool_bwd8(const bf16* __restrict__ x, const bf16* __restrict__ dY, bf16* __restrict__ dX, int B, int H, int W, int C) {
   const int OH = (H + 1) / 2, OW = (W + 1) / 2, C8 = C / 8;
   size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x, n = (size_t)B * H * W * C8;
@@ -463,60 +461,44 @@ extern "C" int gq_bn_relu_bwd(const void* dY, const void* act, const float* o, c
   return 0;
 }
 
-// ------------------------------------------------------------------------------------------------ weight gradient on tcgen05 (r02)
+// ------------------------------------------------------------------------------------------------ weight gradient on wgmma
 // The same contraction as k_wgrad as a tensor-core GEMM:  D[co][ci] (one filter tap, one image) = sum over pixels p of dY[p][co] * X[p + tap][ci],
 // i.e. M = 128 output channels, N = BLOCK_N input channels, K = pixels.  Both operands are pixel-major in memory ([pixel][channel], NHWC), so
-// with K = pixels they are **MN-major** UMMA operands: a shared-memory tile is K rows (pixels) of 128 bytes (64 channels), 8 rows = one
-// 1024-byte swizzle atom - exactly the image a 128-byte-swizzled TMA box of [64 channels x 128 pixels] leaves.  Canonical layout
-// (cute/atom/mma_traits_sm100.hpp, Major-MN, SWIZZLE_128B):  ((8,8,m),(8,k)) : ((1,8,LBO),(64,SBO)) in elements - the next 64 channels
-// (second box) LBO = 16 384 bytes further, the next 8 pixels SBO = 1024 bytes further; one MMA (K = 16) consumes 16 rows = 2048 bytes.
+// with K = pixels they are **MN-major** wgmma operands: a shared-memory tile is K rows (pixels) of 128 bytes (64 channels), 8 rows = one
+// 1024-byte swizzle atom - exactly the image a 128-byte-swizzled TMA box of [64 channels x 128 pixels] leaves.  Canonical MN-major
+// SWIZZLE_128B layout: the next 64 channels (second box) LBO = 16 384 bytes further, the next 8 pixels SBO = 1024 bytes further; one
+// wgmma (K = 16) consumes 16 rows = 2048 bytes.
 //   A = dY: 3-D tiled map [Cout][H*W][B], box 64 x 128 x 1 - rows past the end of the image are out of bounds and read as zeros, so the
 //           last k-step of an image contributes nothing for them whatever the X load returns there;
 //   B = X : the forward's im2col-mode map (tap passed as offsets, zero fill = convolution padding): 128 consecutive output positions.
 // grid (ceil(Cout / 128), Cin / BLOCK_N, taps * B); split-K over the images like k_wgrad (partials [B][Cout][taps][Cin], summed in image
-// order by k_reduce_rows: deterministic).  Roles as in k_conv_tc_tma: warp 0 lane 0 TMA producer, warp 1 lane 0 MMA issuer, warps 2-5
-// read the accumulator (TMEM lane quarter warp % 4 = 32 output channels each) and store it.
+// order by k_reduce_rows: deterministic).  Roles as in k_conv_wgmma: warp 8 lane 0 TMA producer, warpgroup g = 0, 1 multiplies and stores
+// output channels co0 + 64 g .. co0 + 64 g + 63 (its own dY box).
 __device__ __forceinline__ void tma_load_3d(uint32_t dst_smem_addr, const CUtensorMap* tmap, int c0, int c1, int c2, uint64_t* bar) {
   asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4}], [%5];"
                ::"r"(dst_smem_addr), "l"((uint64_t)tmap), "r"(c0), "r"(c1), "r"(c2), "r"(smem_u32(bar)) : "memory");
 }
-// shared-memory matrix descriptor, MN-major, SWIZZLE_128B (see above)
-__device__ __forceinline__ uint64_t make_smem_desc_mn_sw128(uint32_t saddr, uint32_t lbo_bytes) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr >> 4) & 0x3fff);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3fff) << 16;  // leading byte offset: next 64-element atom along M / N
-  d |= (uint64_t)(1024 >> 4) << 32;                  // stride byte offset: next 8 rows along K
-  d |= (uint64_t)1 << 46;                            // descriptor version (Blackwell)
-  d |= (uint64_t)2 << 61;                            // layout type SWIZZLE_128B
-  return d;
-}
 #define WT_K 128                      // pixels per k-step (= the im2col map's pixels per column)
 #define WT_BOX (WT_K * 128)           // bytes of one [64 channels x 128 pixels] box
 template <int BLOCK_N, int STAGES>
-__global__ void __launch_bounds__(192) k_wgrad_tc(const __grid_constant__ CUtensorMap tmap_dy, const __grid_constant__ CUtensorMap tmap_x,
-                                                  float* __restrict__ part, int H, int W, int Cin, int Cout, int ks) {
+__global__ void __launch_bounds__(CONV_THREADS, 1) k_wgrad_wgmma(const __grid_constant__ CUtensorMap tmap_dy, const __grid_constant__ CUtensorMap tmap_x,
+                                                                float* __restrict__ part, int H, int W, int Cin, int Cout, int ks) {
   constexpr int A_STAGE = 2 * WT_BOX, B_STAGE = (BLOCK_N / 64) * WT_BOX;
-  extern __shared__ __align__(1024) uint8_t smem[];
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
   uint8_t* sA = smem;
   uint8_t* sB = smem + STAGES * A_STAGE;
   uint64_t* full = (uint64_t*)(smem + STAGES * (A_STAGE + B_STAGE));
   uint64_t* empty = full + STAGES;
-  uint64_t* acc_full = empty + STAGES;
-  uint32_t* tmem_slot = (uint32_t*)(acc_full + 1);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int taps = ks * ks, pad = ks / 2, HW = H * W, nk = (HW + WT_K - 1) / WT_K;
   const int co0 = blockIdx.x * 128, ci0 = blockIdx.y * BLOCK_N, tap = blockIdx.z % taps, b = blockIdx.z / taps;
   if (tid == 0) {
-    for (int i = 0; i < STAGES; i++) { mbar_init(&full[i], 1); mbar_init(&empty[i], 1); }
-    mbar_init(acc_full, 1);
+    for (int i = 0; i < STAGES; i++) { mbar_init(&full[i], 1); mbar_init(&empty[i], 8); }
     fence_barrier_init();
   }
-  if (warp == 0) tmem_alloc(tmem_slot, BLOCK_N);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tacc = *tmem_slot;
-  if (warp == 0) {
+  if (warp == 8) {
     if (lane == 0) {
       for (int kn = 0; kn < nk; kn++) {
         const int s = kn % STAGES, round = kn / STAGES;
@@ -531,40 +513,38 @@ __global__ void __launch_bounds__(192) k_wgrad_tc(const __grid_constant__ CUtens
           tma_load_im2col_4d(b_dst + (uint32_t)(j * WT_BOX), &tmap_x, ci0 + j * 64, ow0 - pad, oh0 - pad, b, (uint16_t)(tap % ks), (uint16_t)(tap / ks), &full[s]);
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc = make_idesc(128, BLOCK_N) | (1u << 15) | (1u << 16);  // A and B MN-major
-      int s = 0; uint32_t ph = 0;
-      for (int kb = 0; kb < nk; kb++) {
-        mbar_wait(&full[s], ph);
-        tc_fence_after();
-        const uint32_t a_base = smem_u32(sA + s * A_STAGE), b_base = smem_u32(sB + s * B_STAGE);
-#pragma unroll
-        for (int k = 0; k < WT_K / 16; k++)
-          umma_bf16(tacc, make_smem_desc_mn_sw128(a_base + k * 2048, WT_BOX), make_smem_desc_mn_sw128(b_base + k * 2048, WT_BOX), idesc, (kb > 0 || k > 0) ? 1u : 0u);
-        umma_commit(&empty[s]);
-        if (kb == nk - 1) umma_commit(acc_full);
-        if (++s == STAGES) { s = 0; ph ^= 1u; }
-      }
-    }
-  } else {
-    const int quarter = warp & 3, co = co0 + quarter * 32 + lane;
-    mbar_wait(acc_full, 0);
-    tc_fence_after();
-    float* dst_row = part + (((size_t)b * Cout + (co < Cout ? co : 0)) * taps + tap) * Cin + ci0;
-    for (int cb = 0; cb < BLOCK_N; cb += 32) {
-      float v[32];
-      tmem_ld32(tacc + ((uint32_t)(quarter * 32) << 16) + (uint32_t)cb, v);
-      if (co < Cout) {
-        float4* dst = (float4*)(dst_row + cb);
-#pragma unroll
-        for (int j = 0; j < 8; j++) dst[j] = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-      }
-    }
+    return;
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) tmem_dealloc(tacc, BLOCK_N);
+  const int wg = warp >> 2;
+  float acc[BLOCK_N / 2];
+#pragma unroll
+  for (int i = 0; i < BLOCK_N / 2; i++) acc[i] = 0.f;
+  int s = 0, prev = -1;
+  uint32_t ph = 0;
+  for (int kb = 0; kb < nk; kb++) {
+    mbar_wait(&full[s], ph);
+    const uint32_t a_base = smem_u32(sA + s * A_STAGE) + (uint32_t)(wg * WT_BOX), b_base = smem_u32(sB + s * B_STAGE);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < WT_K / 16; k++)
+      wgmma_tile<BLOCK_N, 1, 1>(acc, gmma_desc_sw128(a_base + k * 2048, WT_BOX), gmma_desc_sw128(b_base + k * 2048, WT_BOX), (kb > 0 || k > 0) ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<1>();
+    if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(&empty[prev]); }
+    prev = s;
+    if (++s == STAGES) { s = 0; ph ^= 1u; }
+  }
+  wgmma_wait<0>();
+  // fragment: output channel co0 + 64 wg + 16 (warp % 4) + lane / 4 (+ 8), input channels ci0 + 8 j + 2 (lane % 4) + {0, 1}
+  const int coa = co0 + wg * 64 + (warp & 3) * 16 + (lane >> 2), cob = coa + 8;
+  float* rowa = part + (((size_t)b * Cout + (coa < Cout ? coa : 0)) * taps + tap) * Cin + ci0;
+  float* rowb = part + (((size_t)b * Cout + (cob < Cout ? cob : 0)) * taps + tap) * Cin + ci0;
+#pragma unroll
+  for (int j = 0; j < BLOCK_N / 8; j++) {
+    const int c = 8 * j + 2 * (lane & 3);
+    if (coa < Cout) *(float2*)(rowa + c) = make_float2(acc[4 * j], acc[4 * j + 1]);
+    if (cob < Cout) *(float2*)(rowb + c) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+  }
 }
 
 // 3-D tiled tensor map of dY [B][H*W][Cout] bf16 (innermost first: Cout, H*W, B) with a [64 channels x 128 pixels x 1 image] box
@@ -597,10 +577,10 @@ static int launch_wgrad_tc(cudaStream_t st, const void* dY, const void* x, float
   const int taps = ks * ks;
 #define LAUNCH_WT(BN_, ST_)                                                                                                   \
   do {                                                                                                                        \
-    const size_t smem = (size_t)ST_ * (2 * WT_BOX + (BN_ / 64) * WT_BOX) + 8 * (2 * ST_ + 1) + 16;                              \
-    QCK(cudaFuncSetAttribute(k_wgrad_tc<BN_, ST_>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));                   \
+    const size_t smem = 1024 + (size_t)ST_ * (2 * WT_BOX + (BN_ / 64) * WT_BOX) + 16 * ST_;                                    \
+    QCK(cudaFuncSetAttribute(k_wgrad_wgmma<BN_, ST_>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));                \
     dim3 grid((Cout + 127) / 128, Cin / BN_, taps * B);                                                                       \
-    k_wgrad_tc<BN_, ST_><<<grid, 192, smem, st>>>(tdy, tx, part, H, W, Cin, Cout, ks);                                         \
+    k_wgrad_wgmma<BN_, ST_><<<grid, CONV_THREADS, smem, st>>>(tdy, tx, part, H, W, Cin, Cout, ks);                             \
   } while (0)
   if (Cin % 128 == 0) LAUNCH_WT(128, 3);
   else LAUNCH_WT(64, 4);
@@ -613,7 +593,7 @@ extern "C" int gq_conv_wgrad(const void* dY, const void* x, float* scratch_part,
   if (!dY || !x || !scratch_part || !dW || (ks != 1 && ks != 3) || Cin % 64 || Cout % 64) { snprintf(q_err, sizeof q_err, "gq_conv_wgrad: bad argument"); return -1; }
   cudaStream_t st = (cudaStream_t)stream;
   const int taps = ks * ks;
-  // tcgen05 path by default (GQ_WGRAD_TC=0: the CUDA-core kernel, kept as the A/B partner and for drivers without the tensor-map encoders)
+  // wgmma path by default (GQ_WGRAD_TC=0: the CUDA-core kernel, kept as the A/B partner and for drivers without the tensor-map encoders)
   const char* e_tc = getenv("GQ_WGRAD_TC");  // (read per call: the parity test switches between the two kernels inside one process)
   const int use_tc = (e_tc && atoi(e_tc) == 0) ? 0 : 1;
   int r = use_tc ? launch_wgrad_tc(st, dY, x, scratch_part, B, H, W, Cin, Cout, ks) : 1;

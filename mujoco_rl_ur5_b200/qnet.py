@@ -8,7 +8,7 @@ Grasping_Module_multidiscrete (:243-287)), built from BasicBlock (:92-142) and c
   (`model_state_dict`, Grasping_Agent_multidiscrete.py:560-572) load with `load_state_dict`.  It is a weights container and the
   fp32 comparison target of the tests — the product forward never calls it.
 * `QNetForward` packs the weights once (bf16, [Cout][kh][kw][Cin]) and runs the whole forward with the hand-written kernels:
-  tcgen05 implicit-GEMM convolutions + fused BN/ReLU/residual, max-pool, bilinear up-sampling, sigmoid head, arg-max.
+  wgmma implicit-GEMM convolutions + fused BN/ReLU/residual, max-pool, bilinear up-sampling, sigmoid head, arg-max.
   BatchNorm uses per-image batch statistics: the reference never calls `.eval()` on the policy net and forwards one image at a
   time (SURVEY 3.4, Q9), so a batch of N environments is N independent batch-1 forwards.
 """
@@ -20,7 +20,7 @@ import numpy as np
 _HERE = os.path.dirname(os.path.abspath(__file__))
 QLIB_PATH = os.path.join(_HERE, "csrc", "libgrasp_qnet.so")
 _QLIB = None
-QSYMBOLS = ["gq_last_error", "gq_version", "gq_conv_tc", "gq_conv_tc_block_out", "gq_conv_first", "gq_maxpool", "gq_bn_act", "gq_upsample2x", "gq_head", "gq_head_up2", "gq_argmax", "gq_obs_to_state", "gq_obs_to_state_train"]
+QSYMBOLS = ["gq_last_error", "gq_version", "gq_conv_partials_floats", "gq_conv_tc", "gq_conv_tc_block_out", "gq_conv_first", "gq_maxpool", "gq_bn_act", "gq_upsample2x", "gq_head", "gq_head_up2", "gq_argmax", "gq_obs_to_state", "gq_obs_to_state_train"]
 
 
 def load_qnet_library():
@@ -32,6 +32,8 @@ def load_qnet_library():
         P, I, F = C.c_void_p, C.c_int, C.c_float
         L.gq_last_error.restype = C.c_char_p
         L.gq_version.restype = C.c_char_p
+        L.gq_conv_partials_floats.argtypes = [I, I, I, I]
+        L.gq_conv_partials_floats.restype = C.c_size_t
         L.gq_conv_tc.argtypes = [P, P, P, P, P, P, I, I, I, I, I, I, P]
         L.gq_conv_tc_block_out.argtypes = [P, P, P, P, P, P, P, F, P, P, I, I, I, I, I, I, P]
         L.gq_conv_first.argtypes = [P, P, P, I, I, I, P]
@@ -157,7 +159,7 @@ class QNetForward:
         t = self.torch
         y = t.empty((B, H, W, cout), dtype=t.float32, device=self.dev)
         stats = t.empty((B, cout, 2), dtype=t.float32, device=self.dev) if want_stats else None
-        part = t.empty((B, (H * W + 127) // 128 * 4, cout, 2), dtype=t.float32, device=self.dev) if want_stats else None
+        part = t.empty(self.L.gq_conv_partials_floats(B, H, W, cout), dtype=t.float32, device=self.dev) if want_stats else None
         self._ck(self.L.gq_conv_tc(self._p(x), self._p(w), self._p(bias), self._p(y), self._p(stats), self._p(part), B, H, W, cin, cout, ks, self._stream()), "gq_conv_tc")
         return y, stats
 

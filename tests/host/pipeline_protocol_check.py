@@ -1,22 +1,19 @@
 #!/usr/bin/env python
-"""Model check of the mbarrier protocol of the persistent convolution kernel (k_conv_tc_tma in csrc/qnet.cu = `tma_only`; the
-cp.async-fed variant k_conv_tc_persist modelled by the other mode measured slower in r02a and was deleted from the library).  The
-check was written before either kernel had run on a GPU; both passed their parity tests on the first run.
+"""Model check of the mbarrier protocol of the persistent convolution kernel (k_conv_wgmma in csrc/qnet.cu; k_wgrad_wgmma uses the
+same ring with one tile per CTA).
 
 The kernel's control flow is restated with the SAME index / parity expressions (stage = it % STAGES with a running round counter,
-producer waits empty[s] with parity (round - 1) & 1, the MMA issuer waits full[s] with a phase bit that flips when s wraps, accumulator
-buffer a = i & 1, MMA waits acc_empty[a] with parity ((i >> 1) & 1) ^ 1, epilogue waits acc_full[a] with parity (i >> 1) & 1) and run
-under a randomised scheduler with asynchronous completions (cp.async arrivals, TMA transaction bytes, tcgen05.commit arrivals happen
-"later", in issue order per engine).  mbarriers are modelled with their real semantics: a phase completes when the pending arrival
-count and the pending transaction bytes reach zero, `try_wait.parity P` succeeds iff P differs from the parity of the phase in
-progress - so a waiter that is lapped would be fooled exactly as on hardware.  Checked on every schedule:
+producer waits empty[s] with parity (round - 1) & 1, a consumer waits full[s] with a phase bit that flips when s wraps, and releases a
+stage only after wgmma.wait_group 1 has reported the wgmmas that read it complete) and run under a randomised scheduler with
+asynchronous completions (TMA transaction bytes and wgmma groups complete "later", in issue order per engine).  mbarriers are modelled
+with their real semantics: a phase completes when the pending arrival count and the pending transaction bytes reach zero,
+`try_wait.parity P` succeeds iff P differs from the parity of the phase in progress - so a waiter that is lapped would be fooled
+exactly as on hardware.  Checked on every schedule:
   * no deadlock;
   * every wait passes in the phase it was meant for (no parity aliasing);
-  * a ring stage is overwritten only after the MMAs that read it completed, and is read only when completely filled with the k-step
-    the MMA expects;
-  * an accumulator buffer is accumulated into only after the epilogue of the tile two before has drained it, and is read by the
-    epilogue only when all MMAs of its tile have completed;
-  * every tile is produced, multiplied and drained exactly once, in order.
+  * a ring stage is overwritten only after every consumer's wgmmas that read it completed, and is read only when completely filled
+    with the k-step the consumer expects;
+  * every tile is produced and consumed by every consumer warpgroup exactly once, in order.
 Run: python tests/host/pipeline_protocol_check.py [schedules]
 """
 import random
@@ -50,122 +47,97 @@ class Bar:
         return parity != (self.phase & 1)
 
 
-def simulate(seed, stages, nk, ntiles, nprod=3, nepi=2, b_bytes=64, tma_only=False):
-    """tma_only: k_conv_tc_tma (GQ_PERSIST=2) - one producer thread, both operands by TMA, full barrier count 1 + transaction bytes"""
+def simulate(seed, stages, nk, ntiles, ncons=2, warps_per_cons=4, b_bytes=64):
     rng = random.Random(seed)
-    if tma_only:
-        nprod = 1
-    full = [Bar(1 if tma_only else nprod + 1) for _ in range(stages)]
-    empty = [Bar(1) for _ in range(stages)]
-    acc_full = [Bar(1) for _ in range(2)]
-    acc_empty = [Bar(nepi) for _ in range(2)]
+    full = [Bar(1) for _ in range(stages)]
+    empty = [Bar(ncons * warps_per_cons) for _ in range(stages)]
     # ground truth bookkeeping
-    stage_content = [None] * stages        # (tile, kn) once completely filled
-    stage_fill = [dict() for _ in range(stages)]  # partial fills: (tile, kn) -> set of writers
-    stage_reads_done = [True] * stages     # the MMAs that read the current content have completed
-    acc_tile = [None, None]                # tile whose MMAs are accumulating / have accumulated into the buffer
-    acc_mma_done = [True, True]
-    acc_drained = [[True] * nepi, [True] * nepi]
-    drained_tiles = [[] for _ in range(nepi)]
-    deferred = []                          # asynchronous completions: (engine, callable), executed in order per engine
+    stage_fill = [dict() for _ in range(stages)]  # (tile, kn) -> set of operands landed
+    readers = [set() for _ in range(stages)]      # consumers whose wgmmas reading the stage have not completed
+    consumed = [[] for _ in range(ncons)]
+    reads = {}                                    # (stage, tile, k-step) -> consumers that read it
+    deferred = []                                 # asynchronous completions: (engine, callable), executed in order per engine
+    group_done = [dict() for _ in range(ncons)]   # consumer -> {issue index: completed}
 
-    def defer(engine, fn):
-        deferred.append((engine, fn))
-
-    def producer(pid):
+    def producer():
         sn, rnd = 0, 0
         for t in range(ntiles):
             for kn in range(nk):
                 if rnd > 0:
-                    yield ("wait", empty[sn], (rnd - 1) & 1, rnd - 1, "producer %d empty[%d]" % (pid, sn))
-                # issue the copies of this thread into stage sn (they land later)
-                s_, t_, k_ = sn, t, kn
-
-                def land(s=s_, tt=t_, kk=k_, who=pid):
-                    assert stage_reads_done[s], "stage %d overwritten before its MMAs completed" % s
-                    w = stage_fill[s].setdefault((tt, kk), set())
-                    w.add(("A", who))
-                    full[s].arrive()
-                if tma_only:
-                    full[sn].expect_tx_arrive(2 * b_bytes)
-
-                    def tma_a(s=s_, tt=t_, kk=k_):
-                        assert stage_reads_done[s], "stage %d (activations) overwritten before its MMAs completed" % s
-                        stage_fill[s].setdefault((tt, kk), set()).add(("A", 0))
+                    yield ("wait", empty[sn], (rnd - 1) & 1, rnd - 1, "producer empty[%d]" % sn)
+                full[sn].expect_tx_arrive(2 * b_bytes)
+                for op in ("A", "B"):
+                    def land(s=sn, tt=t, kk=kn, o=op):
+                        assert not readers[s], "stage %d (%s) overwritten before the wgmmas of %s completed" % (s, o, sorted(readers[s]))
+                        for old in [key for key in stage_fill[s] if key != (tt, kk)]:
+                            assert reads.get((s,) + old, 0) == ncons, "stage %d overwritten before every consumer read k-step %s" % (s, old)
+                            del stage_fill[s][old]
+                        stage_fill[s].setdefault((tt, kk), set()).add(o)
                         full[s].complete_tx(b_bytes)
-                    defer("tma", tma_a)
-                elif pid == 0:
-                    full[sn].expect_tx_arrive(b_bytes)
-                if pid == 0:
-                    def tma(s=s_, tt=t_, kk=k_):
-                        assert stage_reads_done[s], "stage %d (weights) overwritten before its MMAs completed" % s
-                        stage_fill[s].setdefault((tt, kk), set()).add(("B", 0))
-                        full[s].complete_tx(b_bytes)
-                    defer("tma", tma)
-                if not tma_only:
-                    defer("cpasync%d" % pid, land)
+                    defer("tma", land)
                 yield ("step",)
                 sn += 1
                 if sn == stages:
                     sn, rnd = 0, rnd + 1
 
-    def mma():
+    def defer(engine, fn):
+        deferred.append((engine, fn))
+
+    def release(c, s):
+        for _ in range(warps_per_cons):  # one arrival per consumer warp after its wgmma.wait_group
+            empty[s].arrive()
+
+    def consumer(c):
         s, ph, it = 0, 0, 0
         for i in range(ntiles):
-            a = i & 1
-            yield ("wait", acc_empty[a], ((i >> 1) & 1) ^ 1, (i >> 1) - 1, "mma acc_empty[%d]" % a)
-            assert all(acc_drained[a]), "accumulator %d reused before the epilogue drained tile %s" % (a, acc_tile[a])
-            acc_tile[a], acc_mma_done[a] = i, False
-            acc_drained[a] = [False] * nepi
+            prev = None
             for kb in range(nk):
-                yield ("wait", full[s], ph, it // stages, "mma full[%d]" % s)
-                fill = stage_fill[s].pop((i, kb), None)
-                assert fill is not None and len(fill) == nprod + 1, "MMA of tile %d k-step %d read stage %d holding %s" % (i, kb, s, fill)
-                assert not stage_fill[s], "stage %d holds copies of another k-step: %s" % (s, stage_fill[s])
-                stage_reads_done[s] = False
+                yield ("wait", full[s], ph, it // stages, "consumer %d full[%d]" % (c, s))
+                fill = stage_fill[s].get((i, kb))
+                assert fill == {"A", "B"}, "consumer %d, tile %d k-step %d read stage %d holding %s" % (c, i, kb, s, stage_fill[s])
+                readers[s].add(c)
+                idx = it
 
-                def done(ss=s):
-                    stage_reads_done[ss] = True
-                    empty[ss].arrive()
-                defer("tensor", done)
-                if kb == nk - 1:
-                    def accdone(aa=a):
-                        acc_mma_done[aa] = True
-                        acc_full[aa].arrive()
-                    defer("tensor", accdone)
+                reads[(s, i, kb)] = reads.get((s, i, kb), 0) + 1
+
+                def done(ss=s, n=idx):
+                    readers[ss].discard(c)
+                    group_done[c][n] = True
+                defer("wgmma%d" % c, done)
                 yield ("step",)
+                # wgmma.wait_group 1: every group but the one just committed has completed
+                if prev is not None:
+                    yield ("until", lambda n=prev[1]: group_done[c].get(n, False), "consumer %d wait_group 1" % c)
+                    release(c, prev[0])
+                prev = (s, idx)
                 it += 1
                 s += 1
                 if s == stages:
                     s, ph = 0, ph ^ 1
+            yield ("until", lambda n=prev[1]: group_done[c].get(n, False), "consumer %d wait_group 0" % c)
+            release(c, prev[0])
+            consumed[c].append(i)
 
-    def epilogue(eid):
-        for i in range(ntiles):
-            a = i & 1
-            yield ("wait", acc_full[a], (i >> 1) & 1, i >> 1, "epilogue %d acc_full[%d]" % (eid, a))
-            assert acc_tile[a] == i and acc_mma_done[a], "epilogue read accumulator %d of tile %s before its MMAs completed" % (a, acc_tile[a])
-            yield ("step",)
-            drained_tiles[eid].append(i)
-            acc_drained[a][eid] = True
-            acc_empty[a].arrive()
-
-    agents = [producer(p) for p in range(nprod)] + [mma()] + [epilogue(e) for e in range(nepi)]
+    agents = [producer()] + [consumer(c) for c in range(ncons)]
     state = [next(g) for g in agents]
     alive = [True] * len(agents)
+
+    def runnable(st):
+        if st[0] == "step":
+            return True
+        if st[0] == "wait":
+            return st[1].ready(st[2])
+        return st[1]()
+
     while any(alive) or deferred:
-        choices = []
-        for k, st in enumerate(state):
-            if not alive[k]:
-                continue
-            if st[0] == "step" or (st[0] == "wait" and st[1].ready(st[2])):
-                choices.append(("agent", k))
+        choices = [("agent", k) for k, st in enumerate(state) if alive[k] and runnable(st)]
         engines = []
         for eng, _ in deferred:
             if eng not in engines:
                 engines.append(eng)  # the oldest completion of every engine may happen now
         choices += [("engine", e) for e in engines]
         if not choices:
-            blocked = [st[4] for k, st in enumerate(state) if alive[k] and st[0] == "wait"]
+            blocked = [st[-1] for k, st in enumerate(state) if alive[k] and st[0] != "step"]
             raise AssertionError("deadlock; blocked: %s" % blocked)
         kind, which = rng.choice(choices)
         if kind == "engine":
@@ -177,15 +149,16 @@ def simulate(seed, stages, nk, ntiles, nprod=3, nepi=2, b_bytes=64, tma_only=Fal
             continue
         st = state[which]
         if st[0] == "wait":
-            bar, parity, intended = st[1], st[2], st[3]
+            bar, intended = st[1], st[3]
             assert bar.phase == intended + 1, "%s passed in phase %d, meant for the completion of phase %d (parity aliasing)" % (st[4], bar.phase, intended)
         try:
             state[which] = next(agents[which])
         except StopIteration:
             alive[which] = False
-    for e in range(nepi):
-        assert drained_tiles[e] == list(range(ntiles))
-    assert all(not f for f in stage_fill)
+    for c in range(ncons):
+        assert consumed[c] == list(range(ntiles))
+    assert all(not r for r in readers)
+    assert all(v == ncons for v in reads.values()) and len(reads) == ntiles * nk
     return True
 
 
@@ -200,9 +173,8 @@ def main():
                     cases += 1
     for r in range(n):
         rr = random.Random(r)
-        simulate(r, rr.choice((3, 4, 6, 8)), rr.choice((1, 4, 9, 18, 36)), rr.choice((1, 2, 4, 7, 9)), nprod=rr.choice((1, 2, 4)), nepi=rr.choice((1, 2, 4)))
-        simulate(r, rr.choice((3, 4, 6, 8)), rr.choice((1, 4, 9, 18, 36)), rr.choice((1, 2, 4, 7, 9)), nepi=rr.choice((1, 2, 4)), tma_only=True)
-        cases += 2
+        simulate(r, rr.choice((2, 3, 4, 6, 8)), rr.choice((1, 4, 9, 18, 36)), rr.choice((1, 2, 4, 7, 9)), ncons=rr.choice((1, 2)))
+        cases += 1
     print("pipeline protocol: %d randomised schedules, no deadlock, no aliasing, no hazard" % cases)
 
 

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Runner used by tests/test_reference_scripts_gpu.py: executes one of the reference's OWN scripts, byte for byte as staged in
-baseline/_ref (or /root/reference), against the B200 engine.  Only loop lengths are shortened, from the OUTSIDE:
+baseline/_ref (or /root/reference), against the H100 engine.  Only loop lengths are shortened, from the OUTSIDE:
 
   example  : example_agent.py (reference: example_agent.py:1-31) has module-level `N_EPISODES = 100` / `N_STEPS = 100`; its source
              text is read, those two literals are replaced IN MEMORY and the result is exec'd (the file is not touched).

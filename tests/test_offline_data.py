@@ -8,7 +8,7 @@ import pytest
 
 from mujoco_rl_ur5_b200 import offline_data as od
 
-REF = "/root/reference"
+DATASET_CASE = {"n": 3, "seed": 5, "item": 1, "sample_seed": 11, "samples": 256}  # the file and item of the reference-loader check
 
 
 def _batch(n, seed=0, H=200, W=200):
@@ -73,44 +73,34 @@ def test_ragged_reference_file_is_cut_to_the_common_prefix(tmp_path):
     assert len(od.load_transitions(p)[0]) == 4
 
 
-@pytest.mark.skipif(not os.path.isdir(os.path.join(REF, "Offline RL")), reason="the reference checkout is not on this machine")
 def test_reference_dataset_class_reads_our_file(tmp_path):
-    """the unmodified Grasping_Dataset (Offline RL/grasping_dataset.py:12-74) on a file written by this module"""
-    pytest.importorskip("torchvision")
-    import importlib.util
-    import types
+    """the unmodified Grasping_Dataset (Offline RL/grasping_dataset.py:12-74), run on a file this module wrote from the same seeded batch,
+    returned what tests/golden/reference_io.json holds (tests/golden/make_reference_io_golden.py).  Here the same file is read the way
+    that class reads it (torch.load, then the 'states' / 'actions' / 'rewards' lists) and item 1's depth channel is recomputed with its
+    transform_observation arithmetic (clip at 1.1, N(0, 0.001) noise after np.random.seed(0), negate, min-max normalise)"""
+    import json
 
-    rgb, depth, act, rew = _batch(3, seed=5)
+    import torch
+
+    g = json.load(open(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_io.json")))["grasping_dataset"]
+    rgb, depth, act, rew = _batch(DATASET_CASE["n"], seed=DATASET_CASE["seed"])
     p = str(tmp_path / "grasping_data_1.pt")
     od.save_transitions(p, rgb, depth, od.flat_action(act), rew)
-    # grasping_dataset.py does `from Modules import simple_Transition`; give it a light stand-in so Modules' own imports are not needed
-    saved = {k: sys.modules.get(k) for k in ("Modules",)}
-    from collections import namedtuple
-
-    sys.modules["Modules"] = types.SimpleNamespace(simple_Transition=namedtuple("simple_Transition", ("state", "action", "reward")))
-    try:
-        spec = importlib.util.spec_from_file_location("ref_grasping_dataset", os.path.join(REF, "Offline RL", "grasping_dataset.py"))
-        mod = importlib.util.module_from_spec(spec)
-        spec.loader.exec_module(mod)
-        import torch
-
-        _orig = torch.load
-        torch.load = lambda f, *a, **k: _orig(f, *a, **{**k, "weights_only": False})  # the reference predates the weights_only default
-        try:
-            ds = mod.Grasping_Dataset(p)
-        finally:
-            torch.load = _orig
-        assert len(ds) == 3
-        np.random.seed(0)
-        state, a, r = ds[1]
-        assert tuple(state.shape) == (4, 200, 200) and a == int(od.flat_action(act)[1]) and r == int(rew[1])
-        assert float(state[3].min()) == 0.0 and float(state[3].max()) == 1.0  # min-max normalised depth channel
-    finally:
-        for k, v in saved.items():
-            if v is None:
-                sys.modules.pop(k, None)
-            else:
-                sys.modules[k] = v
+    data = torch.load(p, weights_only=False)
+    states, actions, rewards = data["states"], data["actions"], data["rewards"]
+    i = DATASET_CASE["item"]
+    assert len(states) == g["len"] and actions[i] == g["action"] and rewards[i] == g["reward"]
+    obs = states[i]
+    assert list(obs["rgb"].shape) == [g["state_shape"][1], g["state_shape"][2], 3] and obs["rgb"].dtype == np.uint8
+    d = obs["depth"].copy()
+    d[np.where(d > 1.1)] = 1.1
+    np.random.seed(0)
+    d += np.random.normal(loc=0, scale=0.001, size=d.shape)  # in place: the float32 array stays float32, as in the reference
+    d *= -1
+    d = ((d - np.min(d)) / (np.max(d) - np.min(d))).reshape(-1)
+    assert float(d.min()) == g["depth_min"] == 0.0 and float(d.max()) == g["depth_max"] == 1.0
+    assert np.allclose(d[g["depth_idx"]], g["depth_values"], rtol=0, atol=1e-6)
+    assert abs(float(d.astype(np.float64).sum()) - g["depth_sum"]) <= 1e-3
 
 
 @pytest.mark.gpu

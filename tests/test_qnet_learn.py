@@ -93,7 +93,7 @@ def _bf(x):
                                              (1, 512, 256, 16, 16)])
 @pytest.mark.parametrize("tc", [1, 0])
 def test_wgrad_and_dgrad_match_autograd(learner, ks, cin, cout, H, W, tc, monkeypatch):
-    """tc = 1: the tcgen05 weight-gradient kernel (default); tc = 0: its CUDA-core A/B partner (GQ_WGRAD_TC=0)"""
+    """tc = 1: the wgmma weight-gradient kernel (default); tc = 0: its CUDA-core A/B partner (GQ_WGRAD_TC=0)"""
     monkeypatch.setenv("GQ_WGRAD_TC", str(tc))
     B = 3
     g = torch.Generator(device="cuda").manual_seed(1)

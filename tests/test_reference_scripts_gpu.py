@@ -1,4 +1,4 @@
-"""Acceptance run of the reference's UNCHANGED scripts against the B200 engine (north star: "... so Grasping_Agent_multidiscrete.py
+"""Acceptance run of the reference's UNCHANGED scripts against the H100 engine (north star: "... so Grasping_Agent_multidiscrete.py
 runs unchanged against it"; VERDICT r01 row N2).
 
 `example_agent.py` (reference: example_agent.py:8-26) and `Grasping_Agent_multidiscrete.main` (:515-583) are executed from the

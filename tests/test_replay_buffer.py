@@ -1,17 +1,16 @@
 """DeviceReplayBuffer (SURVEY 8f.2) against the reference's `Modules.ReplayBuffer` (Modules.py:28-55): same ring behaviour and the
 same sampled transitions from the same `random` stream."""
+import json
 import os
 import random
-import sys
-import types
 
 import numpy as np
-import pytest
 import torch
 
 from mujoco_rl_ur5_b200.replay_buffer import DeviceReplayBuffer
 
-REF = "/root/reference"
+GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_io.json")
+REPLAY_CASES = ((20, 5, 57), (2000, 12, 300), (30, 12, 100))  # (size, batch, pushes)
 
 
 def _drive(buf_push, buf_sample, buf_len, n_push=57, size=20, B=5):
@@ -31,7 +30,7 @@ def _ours(size=20, B=5, n_push=57, rng=None):
 
 
 def test_ring_and_sampling_golden():
-    # generated with the reference class (test below) and frozen here so that the check also runs where /root/reference is absent
+    # = the reference class driven the same way (tests/golden/reference_io.json, first case)
     got = _ours()
     assert got[0] == [2, 4, 1, 6, 9] and got[-1] == [47, 46, 49, 54, 56]  # = Modules.ReplayBuffer(20, simple=True) driven the same way
     again = _ours()
@@ -58,28 +57,13 @@ def test_push_batch_equals_consecutive_pushes():
         assert a.sample_indices(4) == b.sample_indices(4)
 
 
-@pytest.mark.skipif(not os.path.exists(os.path.join(REF, "Modules.py")), reason="the reference checkout is not on this machine")
 def test_same_samples_as_the_reference_class():
-    import importlib.util
-
-    pytest.importorskip("torchvision")
-    saved = sys.modules.get("prettytable")
-    sys.modules["prettytable"] = types.SimpleNamespace(PrettyTable=object)
-    try:
-        spec = importlib.util.spec_from_file_location("ref_modules", os.path.join(REF, "Modules.py"))
-        mod = importlib.util.module_from_spec(spec)
-        spec.loader.exec_module(mod)
-    finally:
-        if saved is None:
-            sys.modules.pop("prettytable", None)
-        else:
-            sys.modules["prettytable"] = saved
-    for size, B, n in ((20, 5, 57), (2000, 12, 300), (30, 12, 100)):
-        rb = mod.ReplayBuffer(size, simple=True)  # seeds the global `random` with 20
-        ref = _drive(lambda k: rb.push(torch.full((1, 1, 2, 2), float(k)), torch.tensor([[k * 3]]), torch.tensor([[k % 2]])),
-                     lambda B_: [int(t.state[0, 0, 0, 0]) for t in rb.sample(B_)], lambda: len(rb), n, size, B)
-        ours = _ours(size, B, n)  # rng=None: the global `random` module, re-seeded with 20 by the constructor
-        assert ours == ref
+    """the reference's Modules.ReplayBuffer(size, simple=True), run unmodified and driven the same way, sampled these transitions
+    (tests/golden/reference_io.json, written by tests/golden/make_reference_io_golden.py); ours draws the same from the same stream"""
+    g = json.load(open(GOLD))["replay_buffer"]
+    assert [(c["size"], c["B"], c["pushes"]) for c in g] == list(REPLAY_CASES)
+    for c in g:
+        assert _ours(c["size"], c["B"], c["pushes"]) == c["samples"]  # rng=None: the global `random` module, re-seeded with 20
 
 
 def test_a_callers_generator_is_not_reseeded():

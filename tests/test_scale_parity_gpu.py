@@ -68,9 +68,12 @@ def test_scene_a_4096_envs_batch_invariance():
     R, N = len(recs), 4096
     assert R == 80
     which = np.arange(N) % R
-    # hand-picked positions: first / last env, both sides of a CTA boundary (4 envs per CTA), both sides of a wave boundary
-    # (148 SMs x 8 resident envs = 1184 envs per wave)
-    for j, e in enumerate([0, 3, 4, 1183, 1184, 2367, 2368, 4092, 4095]):
+    # hand-picked positions: first / last env, both sides of a CTA boundary (4 envs per CTA), both sides of the first two wave boundaries
+    # (SMs x 8 resident envs per wave: 1056 on an H100 SXM)
+    import torch
+
+    wave = torch.cuda.get_device_properties(0).multi_processor_count * 8
+    for j, e in enumerate([0, 3, 4, wave - 1, wave, 2 * wave - 1, 2 * wave, 4092, 4095]):
         which[e] = (7 * j + 16) % R  # rewarded records
     env = BatchedGraspEnv(N, "A", 0)
     env.engine.set_state(np.stack([recs[w]["q0"] for w in which]), np.stack([recs[w]["v0"] for w in which]))

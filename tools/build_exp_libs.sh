@@ -4,13 +4,13 @@
 set -e
 cd "$(dirname "$0")/.."
 CS=mujoco_rl_ur5_b200/csrc
-FLAGS="-gencode arch=compute_100a,code=sm_100a -O3 -lineinfo -std=c++17 -Xcompiler -fPIC -diag-suppress 550"
+FLAGS="-gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -std=c++17 -Xcompiler -fPIC -diag-suppress 550"
 mkdir -p exp_libs/obj
 for L in "$@"; do
   nvcc $FLAGS -DGE_VARIANT=0 $V0FLAGS -c -o exp_libs/obj/v0.o $CS/grasp_engine.cu &
   nvcc $FLAGS -DGE_VARIANT=1 -DGE_BIG_LANES=$L $V1FLAGS -c -o exp_libs/obj/v1_$L.o $CS/grasp_engine.cu &
   nvcc $FLAGS -x cu -c -o exp_libs/obj/d.o $CS/ge_dispatch.cpp &
   wait
-  nvcc -gencode arch=compute_100a,code=sm_100a -shared -o exp_libs/libgrasp_engine_l$L.so exp_libs/obj/v0.o exp_libs/obj/v1_$L.o exp_libs/obj/d.o
+  nvcc -gencode arch=compute_90a,code=sm_90a -shared -o exp_libs/libgrasp_engine_l$L.so exp_libs/obj/v0.o exp_libs/obj/v1_$L.o exp_libs/obj/d.o
   echo built exp_libs/libgrasp_engine_l$L.so
 done

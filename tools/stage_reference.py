@@ -5,7 +5,7 @@
 git-ignored (never committed: the repository holds no reference source) but travels with the snapshot, which is what the bench
 contract reserves it for.  Staged byte for byte: example_agent.py, Grasping_Agent_multidiscrete.py, Modules.py (the agent's
 network + replay buffer) and the pickled `mean_and_std`.  The reference's gym_grasper package is NOT staged: the scripts import
-`gym_grasper` / `gym` from mujoco_rl_ur5_b200/compat, i.e. they run against the B200 engine.
+`gym_grasper` / `gym` from mujoco_rl_ur5_b200/compat, i.e. they run against the H100 engine.
 
   python tools/stage_reference.py [/root/reference]
 """

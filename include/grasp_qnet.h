@@ -32,6 +32,14 @@ int gq_conv_tc(const void* x, const void* w, const float* bias, float* y, float*
  * scratch_scale_shift: B * Cout * 2 floats.  Same shapes and constraints as gq_conv_tc. */
 int gq_conv_tc_block_out(const void* x, const void* w, const float* bias, const float* resid, const float* stats, const float* gamma, const float* beta,
                          float eps, float* scratch_scale_shift, void* out, int B, int H, int W, int Cin, int Cout, int ks, void* stream);
+/* Eval-mode BasicBlock convolutions with BatchNorm folded into the weights (BatchNorm2d with running statistics is a per-channel affine map,
+ * s = gamma * rsqrt(running_var + eps)): out = [relu](conv_ks_a(a, w[:, :ks_a*ks_a*Ca]) + conv1x1(x, w[:, ks_a*ks_a*Ca:]) + bias) as bf16
+ * [B,H,W,Cout], written from the accumulator registers.  a [B,H,W,Ca] bf16; x [B,H,W,Cx] bf16 or NULL (Cx = 0: single source);
+ * w [Cout][ks_a*ks_a*Ca + Cx] bf16 (the [Cout][kh][kw][Ca] weights of the first source followed by the [Cout][Cx] 1x1 weights), bias [Cout]
+ * f32 or NULL.  Per block (Modules.py:126-142): a1 = relu(conv3x3(x, W1 s1) + beta1 - mu1 s1), then
+ * out = relu(conv3x3(a1, W2 s2) + conv1x1(x, W3) + beta2 - mu2 s2 + b3).  Ca, Cx, Cout multiples of 64. */
+int gq_conv_tc_fused(const void* a, const void* x, const void* w, const float* bias, void* out, int relu, int B, int H, int W, int Ca, int Cx, int Cout,
+                     int ks_a, void* stream);
 /* Perception_Module.C1 = conv3x3(4, 64), no bias (Modules.py:163): x [B,4,H,W] f32 NCHW, w [64][3][3][4] f32, y [B,H,W,64] bf16 */
 int gq_conv_first(const float* x, const float* w, void* y, int B, int H, int W, void* stream);
 /* nn.MaxPool2d(kernel_size=3, stride=2, padding=1) (Modules.py:164,166): x [B,H,W,C] -> y [B,ceil(H/2),ceil(W/2),C] */
@@ -74,6 +82,12 @@ int gq_argmax(const float* q, int B, int n, int* idx, float* val, void* stream);
 /* BatchNorm over the whole batch (learn() forwards B images at once, training mode): per-image sums -> batch sums, in place.
  * stats [B,C,2] as written by gq_conv_tc. */
 int gq_bn_batch_merge(float* stats, int B, int C, void* stream);
+/* nn.BatchNorm2d's running-statistics update in a training-mode forward (torch's _BatchNorm.forward with momentum 0.1; the reference's
+ * policy_net(state_batch) in train mode, Grasping_Agent_multidiscrete.py:426 and Offline RL/train.py:109):
+ *   r_mean = (1 - m) r_mean + m mean,  r_var = (1 - m) r_var + m var n / (n - 1),  n = B*HW,
+ * with mean = s1 / HW, var = s2 / HW - mean^2 from merged_stats [B,C,2] as gq_bn_batch_merge leaves them (row 0 is read).  Double
+ * arithmetic, one thread per channel.  running_mean / running_var [C] f32, updated in place. */
+int gq_bn_running_update(const float* merged_stats, float* running_mean, float* running_var, int B, int HW, int C, float momentum, void* stream);
 /* q_pred = net(state).view(B,-1).gather(1, action); loss = binary_cross_entropy(q_pred, reward) (Grasping_Agent_multidiscrete.py:426-443)
  * + backward through sigmoid, the bilinear 2x up-sampling of the head planes and the 1x1 head convolution (Modules.py:250-251,281-283):
  * q [B,A,2H,2W] f32 (forward output), x [B,H,W,64] bf16 (head input), w_head [A,64] f32, action [B] int64 (rot*4HW + y*2W + x), reward [B] f32.

@@ -109,10 +109,11 @@ __device__ __forceinline__ void wgmma_tile(float (&d)[BLOCK_N / 2], uint64_t ade
 //   EPI 0: y = conv + bias (fp32) and, if requested, per-(tile, warp) BatchNorm partials over the warp's 16 rows, reduced over the
 //          lanes in a fixed order (deterministic) and summed in a fixed order by k_bn_reduce
 //   EPI 1 (BasicBlock tail): out = relu(resid * scale + shift + conv + bias) as bf16 (BasicBlock.forward, Modules.py:128-142)
+//   EPI 2 (BatchNorm folded into the weights, eval mode): out = conv + bias as bf16, ReLU if `relu`
 template <int BLOCK_N, int EPI>
 __device__ __forceinline__ void conv_epilogue(const float (&acc)[BLOCK_N / 2], int wg, int warp, int lane, int mt, int n0, int b, int gx, int HW, int Cout,
                                               const float* __restrict__ bias, float* __restrict__ y, float* __restrict__ stats,
-                                              const float* __restrict__ resid, const float2* __restrict__ scale_shift, bf16* __restrict__ out) {
+                                              const float* __restrict__ resid, const float2* __restrict__ scale_shift, bf16* __restrict__ out, int relu) {
   const int wq = warp & 3;
   const int ma = mt * BM + wg * 64 + wq * 16 + (lane >> 2), mb = ma + 8;
   const bool va = ma < HW, vb = mb < HW;
@@ -136,6 +137,10 @@ __device__ __forceinline__ void conv_epilogue(const float (&acc)[BLOCK_N / 2], i
         }
         if (lane < 4) *(float4*)(stats + ((((size_t)b * gx + mt) * CONV_PARTS + wg * 4 + wq) * Cout + c) * 2) = make_float4(s0, q0, s1, q1);
       }
+    } else if constexpr (EPI == 2) {
+      if (relu) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); x2 = fmaxf(x2, 0.f); x3 = fmaxf(x3, 0.f); }
+      if (va) *(__nv_bfloat162*)(out + rowa + c) = __floats2bfloat162_rn(x0, x1);
+      if (vb) *(__nv_bfloat162*)(out + rowb + c) = __floats2bfloat162_rn(x2, x3);
     } else {
       const float4 ss = __ldg((const float4*)(scale_shift + (size_t)b * Cout + c));  // (scale, shift) of columns c, c + 1
       if (va) {
@@ -149,11 +154,15 @@ __device__ __forceinline__ void conv_epilogue(const float (&acc)[BLOCK_N / 2], i
     }
   }
 }
+// Optional second A source (Cx > 0): after the ks*ks taps x Cin/64 chunks of the convolution of x, the K loop runs on over Cx/64 chunks
+// of a 1x1 convolution of x2 (its own im2col map), accumulating into the same registers; the weights are one [Cout][ks*ks*Cin + Cx]
+// matrix, so only the producer's choice of activation map and coordinates depends on the source.
 template <int BLOCK_N, int STAGES, int EPI>
 __global__ void __launch_bounds__(CONV_THREADS, 1) k_conv_wgmma(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant__ CUtensorMap tmap_x,
-                                                               const float* __restrict__ bias, float* __restrict__ y, float* __restrict__ stats,
-                                                               const float* __restrict__ resid, const float2* __restrict__ scale_shift, bf16* __restrict__ out,
-                                                               int H, int W, int Cin, int Cout, int ks, int gx, int gy, int ntiles) {
+                                                               const __grid_constant__ CUtensorMap tmap_x2, const float* __restrict__ bias,
+                                                               float* __restrict__ y, float* __restrict__ stats, const float* __restrict__ resid,
+                                                               const float2* __restrict__ scale_shift, bf16* __restrict__ out, int H, int W, int Cin, int Cx,
+                                                               int Cout, int ks, int relu, int gx, int gy, int ntiles) {
   constexpr int A_STAGE = BM * BK * 2, B_STAGE = BLOCK_N * BK * 2;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);  // the 128-byte swizzle pattern repeats every 1024 bytes
@@ -162,7 +171,7 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) k_conv_wgmma(const __grid_con
   uint64_t* full = (uint64_t*)(smem + STAGES * (A_STAGE + B_STAGE));
   uint64_t* empty = full + STAGES;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int HW = H * W, pad = ks / 2, kchunks = Cin / BK, nk = ks * ks * kchunks;
+  const int HW = H * W, pad = ks / 2, kchunks = Cin / BK, nk_a = ks * ks * kchunks, nk = nk_a + Cx / BK;
   if (tid == 0) {
     for (int i = 0; i < STAGES; i++) { mbar_init(&full[i], 1); mbar_init(&empty[i], 8); }
     fence_barrier_init();
@@ -179,11 +188,15 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) k_conv_wgmma(const __grid_con
         for (int kn = 0; kn < nk; kn++) {
           if (round > 0) mbar_wait(&empty[sn], (uint32_t)(round - 1) & 1u);
           mbar_arrive_expect_tx(&full[sn], (uint32_t)(A_STAGE + B_STAGE));
-          tma_load_im2col_4d(smem_u32(sA) + (uint32_t)(sn * A_STAGE), &tmap_x, kc * BK, ow0 - pad, oh0 - pad, b, (uint16_t)(tap % ks), (uint16_t)(tap / ks),
-                             &full[sn]);
+          if (kn < nk_a) {
+            tma_load_im2col_4d(smem_u32(sA) + (uint32_t)(sn * A_STAGE), &tmap_x, kc * BK, ow0 - pad, oh0 - pad, b, (uint16_t)(tap % ks), (uint16_t)(tap / ks),
+                               &full[sn]);
+            if (++kc == kchunks) { kc = 0; tap++; }
+          } else {
+            tma_load_im2col_4d(smem_u32(sA) + (uint32_t)(sn * A_STAGE), &tmap_x2, (kn - nk_a) * BK, ow0, oh0, b, 0, 0, &full[sn]);
+          }
           tma_load_2d(smem_u32(sB) + (uint32_t)(sn * B_STAGE), &tmap_w, kn * BK, n0, &full[sn]);
           if (++sn == STAGES) { sn = 0; round++; }
-          if (++kc == kchunks) { kc = 0; tap++; }
         }
       }
     }
@@ -214,7 +227,7 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) k_conv_wgmma(const __grid_con
     wgmma_wait<0>();
     __syncwarp();
     if (lane == 0) mbar_arrive(&empty[prev]);
-    conv_epilogue<BLOCK_N, EPI>(acc, wg, warp, lane, mt, nt * BLOCK_N, b, gx, HW, Cout, bias, y, stats, resid, scale_shift, out);
+    conv_epilogue<BLOCK_N, EPI>(acc, wg, warp, lane, mt, nt * BLOCK_N, b, gx, HW, Cout, bias, y, stats, resid, scale_shift, out, relu);
   }
 }
 
@@ -632,7 +645,7 @@ extern "C" int gq_obs_to_state(const unsigned char* rgb, const float* depth, flo
   return 0;
 }
 
-extern "C" const char* gq_version(void) { return "grasp_qnet 0.6 sm_90a bf16 wgmma (persistent CTAs, both operands by TMA: im2col activations + tiled weights, SW128 K-major, register accumulators, fused block tail)"; }
+extern "C" const char* gq_version(void) { return "grasp_qnet 0.7 sm_90a bf16 wgmma (persistent CTAs, both operands by TMA: im2col activations + tiled weights, SW128 K-major, register accumulators, fused block tail, BN-folded dual-source eval blocks)"; }
 
 // tile shape: 128 output pixels x 128 output channels (64 when 128 does not divide Cout); the accumulator of a consumer warpgroup is
 // 64 x BLOCK_N fp32 = BLOCK_N / 2 registers per thread.  One CTA per SM with 192 KB of stages (6 at BLOCK_N 128, 8 at 64): on an H100
@@ -689,15 +702,19 @@ static int make_act_tmap_im2col(CUtensorMap* m, const void* x, int B, int H, int
   return 0;
 }
 
-// EPI 0: y (+ BN partials); EPI 1: out = relu(resid * scale + shift + conv + bias) bf16.  grid = (m tiles, n tiles, images) of the problem.
+// EPI 0: y (+ BN partials); EPI 1: out = relu(resid * scale + shift + conv + bias) bf16; EPI 2: out = [relu](conv + bias) bf16.
+// grid = (m tiles, n tiles, images) of the problem.  x2 / Cx: optional second source, a 1x1 convolution appended to the K loop.
 template <int EPI>
 static int launch_conv(int bn, dim3 grid, cudaStream_t st, const bf16* x, const bf16* w, const float* bias, float* y, float* partials,
-                       const float* resid, const float2* ss, bf16* out, int H, int W, int Cin, int Cout, int ks) {
-  alignas(64) CUtensorMap tm, tmx;
+                       const float* resid, const float2* ss, bf16* out, int H, int W, int Cin, int Cout, int ks, const bf16* x2 = nullptr, int Cx = 0,
+                       int relu = 0) {
+  alignas(64) CUtensorMap tm, tmx, tmx2;
   memset(&tm, 0, sizeof tm);
   memset(&tmx, 0, sizeof tmx);
-  int r = make_weight_tmap(&tm, w, Cout, ks * ks * Cin, bn);
+  memset(&tmx2, 0, sizeof tmx2);
+  int r = make_weight_tmap(&tm, w, Cout, ks * ks * Cin + Cx, bn);
   if (r == 0) r = make_act_tmap_im2col(&tmx, x, (int)grid.z, H, W, Cin, ks);
+  if (r == 0 && Cx > 0) r = make_act_tmap_im2col(&tmx2, x2, (int)grid.z, H, W, Cx, 1);
   if (r) return r;
   int dev = 0, sms = 0;
   QCK(cudaGetDevice(&dev));
@@ -708,7 +725,8 @@ static int launch_conv(int bn, dim3 grid, cudaStream_t st, const bf16* x, const 
   do {                                                                                                                                 \
     const size_t smem = conv_smem(BN_, ST_);                                                                                           \
     QCK(cudaFuncSetAttribute(k_conv_wgmma<BN_, ST_, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));                     \
-    k_conv_wgmma<BN_, ST_, EPI><<<nctas, CONV_THREADS, smem, st>>>(tm, tmx, bias, y, partials, resid, ss, out, H, W, Cin, Cout, ks, gx, gy, ntiles); \
+    k_conv_wgmma<BN_, ST_, EPI><<<nctas, CONV_THREADS, smem, st>>>(tm, tmx, tmx2, bias, y, partials, resid, ss, out, H, W, Cin, Cx, Cout, ks, relu, gx, gy, \
+                                                                   ntiles);                                                            \
   } while (0)
   if (bn == 128) LAUNCH_T(128, 6);
   else LAUNCH_T(64, 8);
@@ -744,6 +762,20 @@ extern "C" int gq_conv_tc_block_out(const void* x, const void* w, const float* b
   dim3 grid((H * W + BM - 1) / BM, Cout / bn, B);
   k_bn_scale_shift<<<(B * Cout + 127) / 128, 128, 0, st>>>(stats, gamma, beta, (float2*)scratch_scale_shift, B, Cout, H * W, eps);
   int r = launch_conv<1>(bn, grid, st, (const bf16*)x, (const bf16*)w, bias, nullptr, nullptr, resid, (const float2*)scratch_scale_shift, (bf16*)out, H, W, Cin, Cout, ks);
+  if (r) return r;
+  QCK(cudaGetLastError());
+  return 0;
+}
+extern "C" int gq_conv_tc_fused(const void* a, const void* x, const void* w, const float* bias, void* out, int relu, int B, int H, int W, int Ca, int Cx,
+                                int Cout, int ks_a, void* stream) {
+  if (!a || !w || !out || (ks_a != 1 && ks_a != 3) || Ca <= 0 || Ca % 64 || Cout <= 0 || Cout % 64 || Cx < 0 || Cx % 64 || (Cx > 0) != (x != nullptr) || B <= 0) {
+    snprintf(q_err, sizeof q_err, "gq_conv_tc_fused: bad argument");
+    return -1;
+  }
+  const int bn = conv_block_n(Cout);
+  dim3 grid((H * W + BM - 1) / BM, Cout / bn, B);
+  int r = launch_conv<2>(bn, grid, (cudaStream_t)stream, (const bf16*)a, (const bf16*)w, bias, nullptr, nullptr, nullptr, nullptr, (bf16*)out, H, W, Ca, Cout, ks_a,
+                         (const bf16*)x, Cx, relu ? 1 : 0);
   if (r) return r;
   QCK(cudaGetLastError());
   return 0;

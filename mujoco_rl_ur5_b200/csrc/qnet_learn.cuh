@@ -30,6 +30,17 @@ __global__ void k_bn_batch_merge(float* __restrict__ stats, int B, int C) {
   const float m1 = (float)(s1 / B), m2 = (float)(s2 / B);
   for (int b = 0; b < B; b++) { stats[((size_t)b * C + c) * 2] = m1; stats[((size_t)b * C + c) * 2 + 1] = m2; }
 }
+// nn.BatchNorm2d's running-statistics update of a training-mode forward (momentum m): from the merged stats (row 0 = batch average of
+// the per-image sums) the batch mean and biased variance the forward normalises with, then r_mean = (1-m) r_mean + m mean and
+// r_var = (1-m) r_var + m var n/(n-1) with n = B*HW values per channel (torch stores the unbiased variance).  One thread per channel.
+__global__ void k_bn_running_update(const float* __restrict__ stats, float* __restrict__ rmean, float* __restrict__ rvar, int C, double HW, double n,
+                                    double m) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= C) return;
+  const double mean = (double)stats[(size_t)c * 2] / HW, var = fmax((double)stats[(size_t)c * 2 + 1] / HW - mean * mean, 0.0);
+  rmean[c] = (float)((1.0 - m) * (double)rmean[c] + m * mean);
+  rvar[c] = (float)((1.0 - m) * (double)rvar[c] + m * var * n / (n - 1.0));
+}
 
 // ------------------------------------------------------------------------------------------------ loss + head backward
 // One CTA per image.  q [B,A,2H,2W] (sigmoid of the bilinearly up-sampled head output), x [B,H,W,64] bf16 (input of the head),
@@ -426,6 +437,15 @@ __global__ void k_adam(float* __restrict__ p, const float* __restrict__ g, float
 extern "C" int gq_bn_batch_merge(float* stats, int B, int C, void* stream) {
   if (!stats || B <= 0 || C <= 0) { snprintf(q_err, sizeof q_err, "gq_bn_batch_merge: bad argument"); return -1; }
   k_bn_batch_merge<<<(C + 127) / 128, 128, 0, (cudaStream_t)stream>>>(stats, B, C);
+  QCK(cudaGetLastError());
+  return 0;
+}
+extern "C" int gq_bn_running_update(const float* merged_stats, float* running_mean, float* running_var, int B, int HW, int C, float momentum, void* stream) {
+  if (!merged_stats || !running_mean || !running_var || B <= 0 || HW <= 0 || C <= 0 || (long long)B * HW < 2) {
+    snprintf(q_err, sizeof q_err, "gq_bn_running_update: bad argument");
+    return -1;
+  }
+  k_bn_running_update<<<(C + 127) / 128, 128, 0, (cudaStream_t)stream>>>(merged_stats, running_mean, running_var, C, (double)HW, (double)B * HW, (double)momentum);
   QCK(cudaGetLastError());
   return 0;
 }

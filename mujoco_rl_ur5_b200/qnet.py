@@ -11,6 +11,9 @@ Grasping_Module_multidiscrete (:243-287)), built from BasicBlock (:92-142) and c
   wgmma implicit-GEMM convolutions + fused BN/ReLU/residual, max-pool, bilinear up-sampling, sigmoid head, arg-max.
   BatchNorm uses per-image batch statistics: the reference never calls `.eval()` on the policy net and forwards one image at a
   time (SURVEY 3.4, Q9), so a batch of N environments is N independent batch-1 forwards.
+* `QNetForward(..., batchnorm="running")` is the eval-mode forward (`policy_net.eval()`, Offline RL/train.py:172): BatchNorm with the
+  running statistics is a per-channel affine map, folded into the convolution weights when they are packed, so a BasicBlock is two
+  wgmma launches (gq_conv_tc_fused) with bf16 outputs and no fp32 intermediates.
 """
 import ctypes as C
 import os
@@ -20,7 +23,7 @@ import numpy as np
 _HERE = os.path.dirname(os.path.abspath(__file__))
 QLIB_PATH = os.path.join(_HERE, "csrc", "libgrasp_qnet.so")
 _QLIB = None
-QSYMBOLS = ["gq_last_error", "gq_version", "gq_conv_partials_floats", "gq_conv_tc", "gq_conv_tc_block_out", "gq_conv_first", "gq_maxpool", "gq_bn_act", "gq_upsample2x", "gq_head", "gq_head_up2", "gq_argmax", "gq_obs_to_state", "gq_obs_to_state_train"]
+QSYMBOLS = ["gq_last_error", "gq_version", "gq_conv_partials_floats", "gq_conv_tc", "gq_conv_tc_block_out", "gq_conv_first", "gq_maxpool", "gq_bn_act", "gq_upsample2x", "gq_head", "gq_head_up2", "gq_argmax", "gq_obs_to_state", "gq_obs_to_state_train", "gq_conv_tc_fused"]
 
 
 def load_qnet_library():
@@ -36,6 +39,7 @@ def load_qnet_library():
         L.gq_conv_partials_floats.restype = C.c_size_t
         L.gq_conv_tc.argtypes = [P, P, P, P, P, P, I, I, I, I, I, I, P]
         L.gq_conv_tc_block_out.argtypes = [P, P, P, P, P, P, P, F, P, P, I, I, I, I, I, I, P]
+        L.gq_conv_tc_fused.argtypes = [P, P, P, P, P, I, I, I, I, I, I, I, I, P]
         L.gq_conv_first.argtypes = [P, P, P, I, I, I, P]
         L.gq_maxpool.argtypes = [P, P, I, I, I, I, P]
         L.gq_bn_act.argtypes = [P, P, P, P, P, P, I, I, I, F, P]
@@ -106,30 +110,60 @@ def make_torch_qnet(number_actions_dim_2=6):
 
 
 _BLOCKS = ["0.RB1", "0.RB2", "0.RB3", "1.RB1", "1.RB2", "1.RB3"]
+BN_EPS = 1e-5
+
+
+def fold_block_weights(sd, name, eps=BN_EPS):
+    """eval-mode BasicBlock `name` with BatchNorm folded into the convolutions, in fp32 (s = gamma * rsqrt(running_var + eps)):
+    -> (w1 [Cout,Cin,3,3] = W1 s1, bias1 [Cout] = beta1 - mu1 s1, w2 [Cout,Cout,3,3] = W2 s2, bias2 [Cout] = beta2 - mu2 s2 + b3)"""
+    s1 = sd[f"{name}.bn1.weight"] * (sd[f"{name}.bn1.running_var"] + eps).rsqrt()
+    s2 = sd[f"{name}.bn2.weight"] * (sd[f"{name}.bn2.running_var"] + eps).rsqrt()
+    w1 = sd[f"{name}.conv1.weight"] * s1[:, None, None, None]
+    w2 = sd[f"{name}.conv2.weight"] * s2[:, None, None, None]
+    b1 = sd[f"{name}.bn1.bias"] - sd[f"{name}.bn1.running_mean"] * s1
+    b2 = sd[f"{name}.bn2.bias"] - sd[f"{name}.bn2.running_mean"] * s2 + sd[f"{name}.conv3.bias"]
+    return w1, b1, w2, b2
 
 
 class QNetForward:
-    """Batched forward on cuda.  `state_dict` uses the reference's key names ('0.C1.weight', '0.RB1.conv1.weight', ...)."""
+    """Batched forward on cuda.  `state_dict` uses the reference's key names ('0.C1.weight', '0.RB1.conv1.weight', ...).
 
-    def __init__(self, state_dict, device=0, max_batch=64):
+    batchnorm="batch" (default): training-mode BatchNorm with each image's own statistics, what the reference's acting forward computes.
+    batchnorm="running": eval-mode BatchNorm with the state_dict's running_mean / running_var (ValueError if it has none), folded into
+    the convolution weights; then the Q-map of an image does not depend on the other images of the batch or on `max_batch`."""
+
+    def __init__(self, state_dict, device=0, max_batch=64, batchnorm="batch"):
         import torch
 
+        if batchnorm not in ("batch", "running"):
+            raise ValueError(f"batchnorm must be 'batch' or 'running', not {batchnorm!r}")
+        if batchnorm == "running":
+            missing = [f"{n}.{bn}.{s}" for n in _BLOCKS for bn in ("bn1", "bn2") for s in ("running_mean", "running_var") if f"{n}.{bn}.{s}" not in state_dict]
+            if missing:
+                raise ValueError(f"batchnorm='running' needs the BatchNorm running statistics; the state_dict has no {missing[0]} (and {len(missing) - 1} more)")
         if not torch.cuda.is_available():
             raise RuntimeError("QNetForward needs a CUDA device (there is no CPU fallback)")
         self.torch = torch
         self.L = load_qnet_library()
         self.dev = torch.device("cuda", device)
         self.max_batch = max_batch
+        self.batchnorm = batchnorm
         sd = {k: v.detach().to(self.dev, torch.float32) for k, v in state_dict.items()}
         self.A = sd["1.C1.weight"].shape[0]
         pack = lambda w: w.permute(0, 2, 3, 1).contiguous().to(torch.bfloat16)  # [Cout,Cin,kh,kw] -> [Cout,kh,kw,Cin]
         self.w_first = sd["0.C1.weight"].permute(0, 2, 3, 1).contiguous()       # [64,3,3,4] f32
         self.blocks = []
         for name in _BLOCKS:
-            b = dict(w1=pack(sd[f"{name}.conv1.weight"]), w2=pack(sd[f"{name}.conv2.weight"]), w3=pack(sd[f"{name}.conv3.weight"]),
-                     b3=sd[f"{name}.conv3.bias"].contiguous(), g1=sd[f"{name}.bn1.weight"].contiguous(), be1=sd[f"{name}.bn1.bias"].contiguous(),
-                     g2=sd[f"{name}.bn2.weight"].contiguous(), be2=sd[f"{name}.bn2.bias"].contiguous(),
-                     cin=sd[f"{name}.conv1.weight"].shape[1], cout=sd[f"{name}.conv1.weight"].shape[0])
+            cin, cout = sd[f"{name}.conv1.weight"].shape[1], sd[f"{name}.conv1.weight"].shape[0]
+            if batchnorm == "running":
+                # folded in fp32, rounded to bf16 once; launch 2's weights are [W2 s2 | W3] = one [Cout][9 Cout + Cin] matrix
+                w1, b1, w2, b2 = fold_block_weights(sd, name)
+                w23 = torch.cat([w2.permute(0, 2, 3, 1).reshape(cout, 9 * cout), sd[f"{name}.conv3.weight"].reshape(cout, cin)], dim=1)
+                b = dict(fw1=pack(w1), fb1=b1.contiguous(), fw23=w23.contiguous().to(torch.bfloat16), fb2=b2.contiguous(), cin=cin, cout=cout)
+            else:
+                b = dict(w1=pack(sd[f"{name}.conv1.weight"]), w2=pack(sd[f"{name}.conv2.weight"]), w3=pack(sd[f"{name}.conv3.weight"]),
+                         b3=sd[f"{name}.conv3.bias"].contiguous(), g1=sd[f"{name}.bn1.weight"].contiguous(), be1=sd[f"{name}.bn1.bias"].contiguous(),
+                         g2=sd[f"{name}.bn2.weight"].contiguous(), be2=sd[f"{name}.bn2.bias"].contiguous(), cin=cin, cout=cout)
             self.blocks.append(b)
         # BasicBlock tail: shortcut conv + BN-apply of the main branch + add + ReLU in one kernel (GQ_FUSE_TAIL=0: separate kernels)
         self.fuse_tail = os.environ.get("GQ_FUSE_TAIL", "1") != "0"
@@ -179,9 +213,20 @@ class QNetForward:
         self._ck(self.L.gq_bn_act(self._p(x), self._p(stats), self._p(gamma), self._p(beta), self._p(identity), self._p(y), B, HW, Cc, 1e-5, self._stream()), "gq_bn_act")
         return y
 
+    def conv_tc_fused(self, a, x, w, bias, B, H, W, ca, cx, cout, ks=3, relu=True):
+        """[relu](conv_ks(a) + conv1x1(x) + bias) -> bf16 [B, H*W, cout] in one wgmma launch; w [cout][ks*ks*ca + cx] bf16, x None when cx = 0"""
+        t = self.torch
+        y = t.empty((B, H * W, cout), dtype=t.bfloat16, device=self.dev)
+        self._ck(self.L.gq_conv_tc_fused(self._p(a), self._p(x), self._p(w), self._p(bias), self._p(y), int(relu), B, H, W, ca, cx, cout, ks, self._stream()),
+                 "gq_conv_tc_fused")
+        return y
+
     def basic_block(self, x, blk, B, H, W):
         """BasicBlock.forward (Modules.py:128-142) on NHWC bf16 `x`"""
         cin, cout = blk["cin"], blk["cout"]
+        if self.batchnorm == "running":
+            a1 = self.conv_tc_fused(x, None, blk["fw1"], blk["fb1"], B, H, W, cin, 0, cout)
+            return self.conv_tc_fused(a1, x, blk["fw23"], blk["fb2"], B, H, W, cout, cin, cout)
         o1, s1 = self.conv_tc(x, blk["w1"], None, B, H, W, cin, cout, 3, True)
         a1 = self.bn_act(o1, s1, blk["g1"], blk["be1"], None, B, H * W, cout)
         o2, s2 = self.conv_tc(a1, blk["w2"], None, B, H, W, cout, cout, 3, True)

@@ -11,12 +11,84 @@ Parameters: fp32 masters under the reference's state_dict names (so checkpoints 
 re-packed after every step; activations bf16, pre-BatchNorm outputs fp32, activation gradients bf16, parameter gradients fp32.
 Multi-GPU data parallel: pass a torch.distributed process group - the parameter gradients (one flat fp32 buffer, 29.3 MB) are summed
 with ONE all-reduce (NCCL over NVLink) between backward and Adam and divided by the world size.
+
+BatchNorm running statistics: every `forward_train` updates the 12 x (running_mean, running_var, num_batches_tracked) buffers as torch's
+training-mode forward does (momentum 0.1, unbiased variance; gq_bn_running_update).  With a process group each rank keeps its own
+running statistics, from its own shard of the batch; write checkpoints from rank 0, which is what DDP's default broadcast_buffers
+amounts to.  The ranks' statistics are not synchronised.
+
+Checkpoints in the reference's format (Offline RL/train.py:84-86,147-163, Grasping_Agent_multidiscrete.py:111-158,561-572):
+`checkpoint()` -> {"model_state_dict", "optimizer_state_dict"}, `QNetLearner.from_checkpoint(ckpt)` restores parameters, buffers and the
+Adam state (m, v, step).  The optimizer part is produced and read by a CPU torch.optim.Adam, so its format is torch's own.
 """
 import ctypes as C
 
 import numpy as np
 
 from .qnet import _BLOCKS, QNetForward, load_qnet_library, make_torch_qnet
+
+BN_MOMENTUM = 0.1  # nn.BatchNorm2d's default, which Modules.py keeps
+_BN_LAYERS = [f"{b}.{bn}" for b in _BLOCKS for bn in ("bn1", "bn2")]
+
+
+def _meta_qnet():
+    """make_torch_qnet(6) without initialising (or drawing random numbers for) its parameters: for the key order and for to_empty()"""
+    import torch
+
+    with torch.device("meta"):
+        return make_torch_qnet(6)
+
+
+def model_keys():
+    """the 87 state_dict keys of Modules.MULTIDISCRETE_RESNET(6) in order (51 parameters, 36 BatchNorm buffers)"""
+    return list(_meta_qnet().state_dict().keys())
+
+
+def _cpu_qnet():
+    import torch
+
+    return _meta_qnet().to_empty(device=torch.device("cpu"))
+
+
+def adam_to_torch(params, m, v, step, lr, betas, eps, weight_decay):
+    """flat Adam state -> torch.optim.Adam(...).state_dict() over make_torch_qnet(6).parameters().  params / m / v: dicts name -> tensor
+    (the reference's parameter names), step: the number of steps taken (0: no per-parameter state yet, as torch leaves it)"""
+    import torch
+
+    net = _cpu_qnet()
+    with torch.no_grad():
+        for k, p in net.named_parameters():
+            p.copy_(params[k].detach().cpu())
+    opt = torch.optim.Adam(net.parameters(), lr=lr, betas=tuple(betas), eps=eps, weight_decay=weight_decay)
+    if step > 0:
+        for k, p in net.named_parameters():
+            opt.state[p] = {"step": torch.tensor(float(step)), "exp_avg": m[k].detach().cpu().clone().to(torch.float32),
+                            "exp_avg_sq": v[k].detach().cpu().clone().to(torch.float32)}
+    return opt.state_dict()
+
+
+def adam_from_torch(opt_state):
+    """torch.optim.Adam state_dict (over make_torch_qnet(6).parameters()) -> (m, v, step, hyper) with m, v dicts name -> CPU tensor
+    (zeros where the optimiser holds no state) and hyper = dict(lr, betas, eps, weight_decay) of its parameter group"""
+    import torch
+
+    net = _cpu_qnet()
+    with torch.no_grad():
+        for p in net.parameters():
+            p.zero_()
+    opt = torch.optim.Adam(net.parameters())
+    opt.load_state_dict(opt_state)
+    m, v, steps = {}, {}, set()
+    for k, p in net.named_parameters():
+        st = opt.state.get(p, {})
+        m[k] = st["exp_avg"].detach().clone() if "exp_avg" in st else torch.zeros_like(p)
+        v[k] = st["exp_avg_sq"].detach().clone() if "exp_avg_sq" in st else torch.zeros_like(p)
+        steps.add(int(float(st["step"])) if "step" in st else 0)
+    if len(steps) != 1:
+        raise ValueError(f"the optimizer state has different step counts per parameter ({sorted(steps)}); the learner keeps one")
+    g = opt.param_groups[0]
+    hyper = dict(lr=float(g["lr"]), betas=tuple(float(b) for b in g["betas"]), eps=float(g["eps"]), weight_decay=float(g["weight_decay"]))
+    return m, v, steps.pop(), hyper
 
 
 def _bind_learn(L):
@@ -32,12 +104,13 @@ def _bind_learn(L):
     L.gq_upsample2x_bwd.argtypes = [P, P, I, I, I, I, P]
     L.gq_add_to_bf16.argtypes = [P, P, P, P, C.c_size_t, P]
     L.gq_adam.argtypes = [P, P, P, P, C.c_size_t, F, F, F, F, F, I, P]
+    L.gq_bn_running_update.argtypes = [P, P, P, I, I, I, F, P]
     L._learn_bound = True
     return L
 
 
 LEARN_SYMBOLS = ["gq_bn_batch_merge", "gq_loss_head_bwd", "gq_bn_relu_bwd", "gq_conv_wgrad", "gq_conv_first_wgrad", "gq_maxpool_bwd", "gq_upsample2x_bwd",
-                 "gq_add_to_bf16", "gq_adam"]
+                 "gq_add_to_bf16", "gq_adam", "gq_bn_running_update"]
 
 
 class QNetLearner:
@@ -67,6 +140,14 @@ class QNetLearner:
             self.p[k] = self.flat[o:o + sz].view(shape)
             self.g[k] = self.grad[o:o + sz].view(shape)
             self.p[k].copy_(state_dict[k].detach().to(self.dev, torch.float32))
+        # BatchNorm buffers, torch's initial values (0 / 1 / 0) where the state_dict has none
+        self.running_mean, self.running_var, self.num_batches_tracked = {}, {}, {}
+        for bn in _BN_LAYERS:
+            c = int(state_dict[f"{bn}.weight"].numel())
+            rm, rv, nb = (state_dict.get(f"{bn}.{s}") for s in ("running_mean", "running_var", "num_batches_tracked"))
+            self.running_mean[bn] = torch.zeros(c, dtype=torch.float32, device=self.dev) if rm is None else rm.detach().to(self.dev, torch.float32).clone()
+            self.running_var[bn] = torch.ones(c, dtype=torch.float32, device=self.dev) if rv is None else rv.detach().to(self.dev, torch.float32).clone()
+            self.num_batches_tracked[bn] = 0 if nb is None else int(nb)
         self.lr, self.wd, self.betas, self.eps = float(lr), float(weight_decay), betas, float(eps)
         self.step_count = 0
         self.pg = process_group
@@ -76,9 +157,58 @@ class QNetLearner:
 
     # ------------------------------------------------------------------ parameters
     def state_dict(self):
-        """fp32 parameters under the reference's names (BatchNorm running statistics are not tracked: the reference never uses them -
-        the policy net is never put in eval mode, Q9)"""
+        """fp32 parameters under the reference's names (parameters only; `model_state_dict()` adds the BatchNorm buffers)"""
         return {k: v.detach().clone() for k, v in self.p.items()}
+
+    def model_state_dict(self):
+        """the full state_dict of Modules.MULTIDISCRETE_RESNET(6): 51 parameters and 36 BatchNorm buffers, CPU fp32 (num_batches_tracked
+        int64), in the module's key order - loads with strict=True into the reference's network"""
+        t = self.torch
+        out = {}
+        for k in model_keys():
+            bn, _, leaf = k.rpartition(".")
+            if k in self.p:
+                out[k] = self.p[k].detach().cpu().clone()
+            elif leaf == "running_mean":
+                out[k] = self.running_mean[bn].detach().cpu().clone()
+            elif leaf == "running_var":
+                out[k] = self.running_var[bn].detach().cpu().clone()
+            elif leaf == "num_batches_tracked":
+                out[k] = t.tensor(self.num_batches_tracked[bn], dtype=t.int64)
+            else:
+                raise KeyError(k)
+        return out
+
+    def checkpoint(self):
+        """{"model_state_dict", "optimizer_state_dict"} as the reference saves them (Offline RL/train.py:147-163); the optimizer part is
+        torch.optim.Adam's own state_dict (step, exp_avg = m, exp_avg_sq = v; lr / betas / eps / weight_decay)"""
+        return {"model_state_dict": self.model_state_dict(),
+                "optimizer_state_dict": adam_to_torch(self.p, self._flat_views(self.m), self._flat_views(self.v), self.step_count, self.lr, self.betas,
+                                                      self.eps, self.wd)}
+
+    @classmethod
+    def from_checkpoint(cls, ckpt, device=0, **kw):
+        """learner from a {"model_state_dict", "optimizer_state_dict"} checkpoint (written by `checkpoint()` or by the reference's scripts):
+        parameters, BatchNorm buffers, Adam moments and step count; lr / betas / eps / weight_decay from the optimizer's parameter group
+        unless given in `kw`.  A checkpoint without "optimizer_state_dict" starts a fresh optimiser."""
+        opt = ckpt.get("optimizer_state_dict")
+        if opt is None:
+            return cls(ckpt["model_state_dict"], device, **kw)
+        m, v, step, hyper = adam_from_torch(opt)
+        L = cls(ckpt["model_state_dict"], device, **{**hyper, **kw})
+        mv, vv = L._flat_views(L.m), L._flat_views(L.v)
+        for k in L.names:
+            mv[k].copy_(m[k].to(L.dev, L.torch.float32))
+            vv[k].copy_(v[k].to(L.dev, L.torch.float32))
+        L.step_count = step
+        return L
+
+    def _flat_views(self, flat):
+        return {k: flat[int(o):int(o) + self.p[k].numel()].view(self.p[k].shape) for k, o in zip(self.names, self.offsets[:-1])}
+
+    def eval_forward(self, max_batch=64):
+        """QNetForward in eval mode (batchnorm="running", BatchNorm folded into the weights) from the current parameters and buffers"""
+        return QNetForward(self.model_state_dict(), self.dev.index or 0, max_batch=max_batch, batchnorm="running")
 
     def _repack(self):
         """bf16 kernel layouts from the fp32 masters: the forward's [Cout][kh][kw][Cin] (QNetForward) and, for the input-gradient
@@ -114,20 +244,29 @@ class QNetLearner:
     def _merge(self, stats, B, Cc):
         self._ck(self.L.gq_bn_batch_merge(self._p(stats), B, Cc, self._st()), "gq_bn_batch_merge")
 
+    def _running_update(self, bn, stats, B, HW, Cc):
+        """torch's training-mode buffer update of BatchNorm layer `bn` from its merged batch statistics"""
+        self._ck(self.L.gq_bn_running_update(self._p(stats), self._p(self.running_mean[bn]), self._p(self.running_var[bn]), B, HW, Cc, BN_MOMENTUM, self._st()),
+                 "gq_bn_running_update")
+        self.num_batches_tracked[bn] += 1
+
     # ------------------------------------------------------------------ forward over the batch (training mode), activations kept
-    def _block_fwd(self, x, blk, B, H, W):
+    def _block_fwd(self, x, blk, B, H, W, name):
         fw = self.fw
         cin, cout = blk["cin"], blk["cout"]
         o1, s1 = fw.conv_tc(x, blk["w1"], None, B, H, W, cin, cout, 3, True)
         self._merge(s1, B, cout)
+        self._running_update(f"{name}.bn1", s1, B, H * W, cout)
         a1 = fw.bn_act(o1, s1, blk["g1"], blk["be1"], None, B, H * W, cout)
         o2, s2 = fw.conv_tc(a1, blk["w2"], None, B, H, W, cout, cout, 3, True)
         self._merge(s2, B, cout)
+        self._running_update(f"{name}.bn2", s2, B, H * W, cout)
         out = fw.conv_tc_block_out(x, blk["w3"], blk["b3"], o2, s2, blk["g2"], blk["be2"], B, H, W, cin, cout, 1)
         return out, dict(x=x, o1=o1, s1=s1, a1=a1, o2=o2, s2=s2, out=out, H=H, W=W)
 
     def forward_train(self, state):
-        """state [B,4,H,W] f32 -> (q [B,A,H,W] f32, saved activations)"""
+        """state [B,4,H,W] f32 -> (q [B,A,H,W] f32, saved activations).  Updates the BatchNorm running statistics, as torch's
+        training-mode forward does."""
         t, fw = self.torch, self.fw
         state = state.to(self.dev, t.float32).contiguous()
         B, _, H, W = state.shape
@@ -135,15 +274,15 @@ class QNetLearner:
         fw._ck(fw.L.gq_conv_first(fw._p(state), fw._p(fw.w_first), fw._p(x0), B, H, W, fw._stream()), "gq_conv_first")
         h, w = (H + 1) // 2, (W + 1) // 2
         p0 = fw.maxpool(x0, B, H, W, 64)
-        b0, sv0 = self._block_fwd(p0, fw.blocks[0], B, h, w)
+        b0, sv0 = self._block_fwd(p0, fw.blocks[0], B, h, w, _BLOCKS[0])
         h2, w2 = (h + 1) // 2, (w + 1) // 2
         p1 = fw.maxpool(b0.view(B, h, w, 128), B, h, w, 128)
-        b1, sv1 = self._block_fwd(p1, fw.blocks[1], B, h2, w2)
-        b2, sv2 = self._block_fwd(b1, fw.blocks[2], B, h2, w2)
-        b3, sv3 = self._block_fwd(b2, fw.blocks[3], B, h2, w2)
-        b4, sv4 = self._block_fwd(b3, fw.blocks[4], B, h2, w2)
+        b1, sv1 = self._block_fwd(p1, fw.blocks[1], B, h2, w2, _BLOCKS[1])
+        b2, sv2 = self._block_fwd(b1, fw.blocks[2], B, h2, w2, _BLOCKS[2])
+        b3, sv3 = self._block_fwd(b2, fw.blocks[3], B, h2, w2, _BLOCKS[3])
+        b4, sv4 = self._block_fwd(b3, fw.blocks[4], B, h2, w2, _BLOCKS[4])
         u0 = fw.upsample(b4.view(B, h2, w2, 128), B, h2, w2, 128)
-        b5, sv5 = self._block_fwd(u0, fw.blocks[5], B, 2 * h2, 2 * w2)
+        b5, sv5 = self._block_fwd(u0, fw.blocks[5], B, 2 * h2, 2 * w2, _BLOCKS[5])
         A = fw.A
         q = t.empty((B, A, 4 * h2, 4 * w2), dtype=t.float32, device=self.dev)
         z = t.empty((B, A, 2 * h2, 2 * w2), dtype=t.float32, device=self.dev)
@@ -257,9 +396,10 @@ class QNetLearner:
         return loss_terms.mean(), qsel
 
     # ------------------------------------------------------------------ one learn() call
-    def learn_step(self, state, action, reward):
+    def learn_step(self, state, action, reward, return_pred=False):
         """state [B,4,H,W] f32 (what the agent stores in its replay buffer), action [B] or [B,1] flat indices rot*H*W + y*W + x, reward [B] or
-        [B,1].  Returns the loss as a float (one device->host read, like the reference's `loss.item()`)."""
+        [B,1].  Returns the loss as a float (one device->host read, like the reference's `loss.item()`); with return_pred=True
+        (loss, q_pred [B] on the device), q_pred being the gathered Q-values of the training forward (Offline RL/train.py:109,122)."""
         t = self.torch
         q, saved = self.forward_train(state)
         works = []
@@ -274,11 +414,11 @@ class QNetLearner:
             def on_ready(prefix):
                 works.append(dist.all_reduce(self.grad_slice(prefix), op=dist.ReduceOp.AVG, group=self.pg, async_op=True))
 
-        loss, _ = self.backward(q, saved, action, reward, on_ready)
+        loss, qsel = self.backward(q, saved, action, reward, on_ready)
         for w in works:
             w.wait()  # (stream-level wait: Adam below is ordered after the last piece)
         self.step_count += 1
         self._ck(self.L.gq_adam(self._p(self.flat), self._p(self.grad), self._p(self.m), self._p(self.v), self.flat.numel(), self.lr, self.betas[0], self.betas[1],
                                 self.eps, self.wd, self.step_count, self._st()), "gq_adam")
         self._repack()
-        return float(loss)
+        return (float(loss), qsel) if return_pred else float(loss)

@@ -91,7 +91,8 @@ int gq_bn_running_update(const float* merged_stats, float* running_mean, float* 
 /* q_pred = net(state).view(B,-1).gather(1, action); loss = binary_cross_entropy(q_pred, reward) (Grasping_Agent_multidiscrete.py:426-443)
  * + backward through sigmoid, the bilinear 2x up-sampling of the head planes and the 1x1 head convolution (Modules.py:250-251,281-283):
  * q [B,A,2H,2W] f32 (forward output), x [B,H,W,64] bf16 (head input), w_head [A,64] f32, action [B] int64 (rot*4HW + y*2W + x), reward [B] f32.
- * Out: loss_terms [B] (mean = the loss), qsel [B] = q_pred, dX [B,H,W,64] bf16, dW_head [A,64], db_head [A]; partials [B,A,64], [B,A]. */
+ * Out: loss_terms [B] (mean = the loss), qsel [B] = q_pred, dX [B,H,W,64] bf16, dW_head [A,64], db_head [A]; partials [B,A,64], [B,A].
+ * As in torch's fp32 autograd, an image whose q_pred is exactly 0 or 1 contributes loss 100 (or 0) and no gradient. */
 int gq_loss_head_bwd(const float* q, const void* x, const float* w_head, const long long* action, const float* reward, int B, int A, int H, int W,
                      float* loss_terms, float* qsel, void* dX, float* dW_partial, float* db_partial, float* dW_head, float* db_head, void* stream);
 /* backward of y = relu(BatchNorm(o) [+ identity]) with batch statistics (BasicBlock, Modules.py:128-142): dY, act = y [B,HW,C] bf16, o [B,HW,C] f32,

@@ -44,7 +44,9 @@ __global__ void k_bn_running_update(const float* __restrict__ stats, float* __re
 
 // ------------------------------------------------------------------------------------------------ loss + head backward
 // One CTA per image.  q [B,A,2H,2W] (sigmoid of the bilinearly up-sampled head output), x [B,H,W,64] bf16 (input of the head),
-// action [B] = rot * (2H*2W) + y * 2W + x, reward [B].  With v = pre-sigmoid value at the chosen pixel: dL/dv = (q - r) / B.
+// action [B] = rot * (2H*2W) + y * 2W + x, reward [B].  With v = pre-sigmoid value at the chosen pixel, dL/dv follows torch's chain
+// rule in fp32: BCE backward (q - r) / B / max(q (1 - q), 1e-12), then the sigmoid's q (1 - q).  Mathematically that is (q - r) / B, but
+// where q rounds to exactly 1 or 0 (logit above ~16.6 or below ~-88) torch's gradient is 0 (the loss is clamped at 100), and so is this one.
 // v = UP2(z)[rot, y, x] = sum of 4 bilinear taps of z = W_head x + b on the H x W map, so the gradient reaches 4 (or fewer) pixels:
 //   dx[pix,:] += g w W_head[rot,:],  dW_head[rot,:] += g w x[pix,:],  db_head[rot] += g w.
 // Outputs: loss_terms [B] (-(r log q + (1-r) log(1-q)), logs clamped at -100 like torch), dX [B,H,W,64] bf16 (zero-filled by the
@@ -62,7 +64,8 @@ __global__ void __launch_bounds__(64) k_loss_head_bwd(const float* __restrict__ 
     loss_terms[b] = -(r * fmaxf(logf(qv), -100.f) + (1.f - r) * fmaxf(logf(1.f - qv), -100.f));
     qsel[b] = qv;
   }
-  const float g = (qv - r) / (float)B;
+  const float sg = (1.f - qv) * qv;
+  const float g = (1.f / (float)B) * (qv - r) / fmaxf(sg, 1e-12f) * sg;
   const float fy = oy * (float)(H - 1) / (float)(OH - 1), fx = ox * (float)(W - 1) / (float)(OW - 1);
   const int y0 = (int)fy, x0 = (int)fx, y1 = min(y0 + 1, H - 1), x1 = min(x0 + 1, W - 1);
   const float wy = fy - y0, wx = fx - x0;

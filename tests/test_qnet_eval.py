@@ -127,14 +127,20 @@ def test_bn_running_update_matches_float64():
 
 @gpu
 def test_learner_running_statistics_match_torch_train_forward():
-    """one learn_step on the golden batch of test_qnet_learn: the 36 buffers against torch's train()-mode forward of the fp32 net on the
-    same batch; relative error no worse than 1.1 x what torch's own autocast-bf16 forward makes + 0.01"""
+    """one learn_step on a batch of test_qnet_learn at each B = 3 (the golden batch), 1, 12 (the reference's BATCH_SIZE) and 15 (the offline
+    trainer's): the 36 buffers against torch's train()-mode forward of the fp32 net on the same batch; relative error no worse than
+    1.1 x what torch's own autocast-bf16 forward makes + 0.01"""
+    for B in (3, 1, 12, 15):
+        _check_running_statistics(B)
+
+
+def _check_running_statistics(B):
     sys.path.insert(0, HERE)
-    from test_qnet_learn import _golden_batch, rel
+    from test_qnet_learn import _batch, rel
 
     from mujoco_rl_ur5_b200.qnet_learn import QNetLearner
 
-    state, action, reward = _golden_batch()
+    state, action, reward = _batch(B)
     net = _net(0)
     L = QNetLearner(net.state_dict(), 0)
     L.learn_step(state, action, reward)
@@ -148,9 +154,9 @@ def test_learner_running_statistics_match_torch_train_forward():
     for k in sd32:
         if "running" in k:
             e, a = rel(ours[k], sd32[k].cpu()), rel(sd16[k].cpu(), sd32[k].cpu())
-            assert e <= 1.1 * a + 0.01, (k, e, a)
+            assert e <= 1.1 * a + 0.01, (B, k, e, a)
         elif "num_batches" in k:
-            assert int(ours[k]) == int(sd32[k]) == 1 and ours[k].dtype == torch.int64
+            assert int(ours[k]) == int(sd32[k]) == 1 and ours[k].dtype == torch.int64, (B, k)
 
 
 def _ref_conv(a, w, bias, ks, relu, x=None, w3=None):

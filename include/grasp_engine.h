@@ -44,7 +44,10 @@ int ge_destroy(ge_handle h);
 
 /* model sizes: what = 0 nq, 1 nv, 2 nbody, 3 ngeom, 4 nu, 5 n_envs, 6 max contacts per env, 7 shared-memory bytes per env,
  * 8 environments (warps) per CTA of the sub-step kernel, 9 workspace placement (0 shared memory, 1 HBM rows: scenes whose per-env
- * workspace exceeds 227 KB, e.g. the 40-object scene) */
+ * workspace exceeds 227 KB, e.g. the 40-object scene), 10 hcap = doubles of the Newton Hessian block region in the workspace, 11 hfull =
+ * nv (nv + 1) / 2 = doubles of one env's Hessian overflow row in HBM (CTA-per-env build: a Hessian build whose blocks add up to more
+ * than hcap goes there).  The CTA-per-env build reads two overrides at ge_create: GE_MAXCON (contact capacity, 16..512) and GE_HCAP
+ * (hcap, from Σ tree blocks + 6 maxcon + 64 up to hfull); a value outside its range is ignored, so size 6 / 10 tell what was used. */
 int ge_size(ge_handle h, int what);
 
 /* MujocoEnv.set_state + controller re-sync, as GraspEnv.reset_model does (GraspingEnv.py:466-470):
@@ -114,7 +117,12 @@ int ge_render(ge_handle h, int cam, int width, int height, uint8_t* rgb, float* 
 
 /* diagnostics for parity tests: copies one internal per-env field of env `env` to a host buffer after running the
  * forward pipeline once on the current state (no integration).  field: "xpos","xmat","cdof","qM","qfrc_bias",
- * "qacc_smooth","qacc","qfrc_constraint","contact" (16 doubles per contact: dist,pos3,frame9,geom1,geom2,dim), "ncon","niter".
+ * "qacc_smooth","qacc","qfrc_constraint","contact" (16 doubles per contact: dist,pos3,frame9,geom1,geom2,dim), "ncon","niter","nsr",
+ * "status" (the status word this forward pass produced, bits as for ge_get_status), "ncand" (broad-phase survivors, counted before
+ * the candidate list is cut at 2 x max contacts), "nmpr" (MPR pairs among the kept candidates),
+ * "hlayout" (the last Newton Hessian build; nothing when the solve had no constraint rows): [hflag (1: blocks in the HBM overflow row),
+ * total block doubles, ntree, then per tree: coupled (0/1), island label (smallest member tree; own index when uncoupled), owner warp
+ * (CTA-per-env build, coupled trees; else -1), block offset, rows of its block (tree dofs, or island dofs when coupled)].
  * Returns the number of doubles written (<= cap) or a negative error. */
 int ge_debug_forward(ge_handle h, int env, const char* field, double* out /*[host]*/, int cap);
 

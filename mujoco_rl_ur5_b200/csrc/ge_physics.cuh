@@ -727,12 +727,14 @@ __device__ __forceinline__ void make_frame(double* fr) {
 // Broad phase over the static candidate pair list (bounding spheres, then oriented boxes), analytic narrow phase one lane
 // per surviving pair, then the MPR pairs, each with one whole warp (the warps of a CTA-per-env build take them round-robin).
 // Returns the number of contacts; sets bit 0 of *status on overflow.  (The oracle emits contacts in the same order: analytic
-// pairs first, then MPR pairs, both in candidate order.)
+// pairs first, then MPR pairs, both in candidate order.)  A list that overflows keeps the first maxcon contacts of that order.
 __device__ __forceinline__ bool pair_is_analytic(int t1, int t2) {
   return (t1 == G_PLANE) || (t1 == G_SPHERE && (t2 == G_SPHERE || t2 == G_BOX || t2 == G_CAPSULE || t2 == G_CYLINDER)) ||
          (t1 == G_BOX && t2 == G_BOX) || (t1 == G_CAPSULE && t2 == G_CAPSULE);
 }
-__device__ __noinline__ int stage_collision(double* ws, int* wi, int lane, int* status) {
+// what one collision stage found: contacts kept, broad-phase survivors (before the maxcand cut), MPR pairs among the kept candidates
+struct CollisionCounts { int ncon, ncand, nmpr; };
+__device__ __noinline__ CollisionCounts stage_collision(double* ws, int* wi, int lane, int* status) {
   const DevModel& m = c_m; const Layout& L = c_L;
   const double *gpos = ws + L.gpos, *gmat = ws + L.gmat, *gcen = ws + L.gcen;
   const int wl = lane & 31, wid = lane >> 5;
@@ -766,6 +768,7 @@ __device__ __noinline__ int stage_collision(double* ws, int* wi, int lane, int* 
     if (pass && pos < L.maxcand) cand[pos] = p;
     ncand += total;
   }
+  const int nsurv = ncand;
   if (ncand > L.maxcand) { ncand = L.maxcand; *status |= 1; }
   gsync();
   double* con = ws + L.con;
@@ -819,16 +822,20 @@ __device__ __noinline__ int stage_collision(double* ws, int* wi, int lane, int* 
   if (ncon > L.maxcon) { ncon = L.maxcon; *status |= 1; }
   gsync();
   // ---- convex pairs through MPR
+  int nmpr = 0;
 #if GE_NW == 1
+  bool full = false;  // a hit found no room: the rest of the MPR pairs are only counted
   for (int ci = 0; ci < ncand; ci++) {
     int p = cand[ci];
     int g1 = m.pair_geom[2 * p], g2 = m.pair_geom[2 * p + 1], t1 = m.geom_type[g1], t2 = m.geom_type[g2];
     if (pair_is_analytic(t1, t2)) continue;
+    nmpr++;
+    if (full) continue;
     double margin = m.pair_margin[p], depth, dir[3], pos[3];
     if (!mpr_w(ws, g1, g2, 0.5 * margin, &depth, dir, pos, lane)) continue;
     double dist = margin - depth;
     if (dist >= margin) continue;
-    if (ncon >= L.maxcon) { *status |= 1; break; }
+    if (ncon >= L.maxcon) { *status |= 1; full = true; continue; }
     if (lane == 0) {
       double* c = con + ncon * L.cstride;
       c[C_DIST] = dist; v3copy(c + C_POS, pos); v3copy(c + C_FRAME, dir);
@@ -839,58 +846,81 @@ __device__ __noinline__ int stage_collision(double* ws, int* wi, int lane, int* 
   gsync();
 #else
   {
-    // every warp walks the whole candidate list and takes the MPR pairs k = wid, wid + GE_NW, ...; MPR pair number k writes its
-    // result into contact slot ncon + k (cpair = -1: no contact), then the slots are compacted in order
-    int k = 0;
+    // Rounds: with `room` = maxcon - ncon free slots, the next (at most room) MPR pairs are dealt out, pair number k of the stage to
+    // warp k % GE_NW; the j-th pair of the round writes its result into contact slot ncon + j (cpair = -1: no contact), then the slots
+    // are compacted in order.  A round whose pairs missed leaves room for the next one, so the list ends as the first maxcon contacts
+    // of the emission order.  Normally every MPR pair fits the first round (one round, three barriers).  Once the list is full, the
+    // remaining pairs are only tested for a hit, which is an overflow.
+    int k = 0, ci = 0;
     bool overflow = false;
-    for (int ci = 0; ci < ncand; ci++) {
-      int p = cand[ci];
-      int g1 = m.pair_geom[2 * p], g2 = m.pair_geom[2 * p + 1], t1 = m.geom_type[g1], t2 = m.geom_type[g2];
-      if (pair_is_analytic(t1, t2)) continue;
-      const int slot = ncon + k;
-      const bool mine = (k % GE_NW) == wid;
-      k++;
-      if (slot >= L.maxcon) { overflow = true; continue; }
-      if (!mine) continue;
-      double margin = m.pair_margin[p], depth = 0, dir[3], pos[3];
-      bool hit = mpr_w(ws, g1, g2, 0.5 * margin, &depth, dir, pos, wl);
-      double dist = margin - depth;
-      if (hit && dist >= margin) hit = false;
-      if (wl == 0) {
-        double* c = con + slot * L.cstride;
-        if (hit) { c[C_DIST] = dist; v3copy(c + C_POS, pos); v3copy(c + C_FRAME, dir); }
-        cpair[slot] = hit ? p : -1;
-      }
-    }
-    gsync();
-    int nslots = ncon + k < L.maxcon ? ncon + k : L.maxcon;
-    // every thread counts the hits first (read-only), THEN warp 0 alone compacts in place: record j moves down to the next free slot
-    // (never overtakes an unread record).  (r02d: a version in which all threads walked the flags while warp 0 was already moving
-    // records let a slow thread read a flag that had just been overwritten - its contact count then differed from the others';
-    // found by racecheck once the workspace was in shared memory.)
-    int nhit = 0;
-    for (int j = ncon; j < nslots; j++) nhit += cpair[j] >= 0;
-    gsync();
-    if (wid == 0) {
-      int o2 = ncon;
-      for (int j = ncon; j < nslots; j++) {
-        const int p = cpair[j];
-        __syncwarp();  // every lane has read flag j before lane 0 may overwrite a lower slot
-        if (p < 0) continue;
-        if (o2 != j) {
-          for (int q = wl; q < C_FRAME + 3; q += 32) con[o2 * L.cstride + q] = con[j * L.cstride + q];
-          if (wl == 0) cpair[o2] = p;
+    for (;;) {
+      const int room = L.maxcon - ncon, k0 = k;
+      if (room <= 0) {
+        bool hit_any = false;
+        for (; ci < ncand; ci++) {
+          int p = cand[ci];
+          int g1 = m.pair_geom[2 * p], g2 = m.pair_geom[2 * p + 1], t1 = m.geom_type[g1], t2 = m.geom_type[g2];
+          if (pair_is_analytic(t1, t2)) continue;
+          const bool mine = (k % GE_NW) == wid;
+          k++;
+          if (!mine || hit_any) continue;
+          double margin = m.pair_margin[p], depth = 0, dir[3], pos[3];
+          const bool hit = mpr_w(ws, g1, g2, 0.5 * margin, &depth, dir, pos, wl) && margin - depth < margin;
+          hit_any = __any_sync(FULL, hit) != 0;  // (warp-uniform: the warp's later pairs are skipped together)
         }
-        o2++;
+        overflow |= group_any(hit_any);
+        break;
       }
-    }
-    const int out = ncon + nhit;
+      for (; ci < ncand; ci++) {
+        int p = cand[ci];
+        int g1 = m.pair_geom[2 * p], g2 = m.pair_geom[2 * p + 1], t1 = m.geom_type[g1], t2 = m.geom_type[g2];
+        if (pair_is_analytic(t1, t2)) continue;
+        if (k - k0 >= room) break;  // this pair opens the next round
+        const int slot = ncon + k - k0;
+        const bool mine = (k % GE_NW) == wid;
+        k++;
+        if (!mine) continue;
+        double margin = m.pair_margin[p], depth = 0, dir[3], pos[3];
+        bool hit = mpr_w(ws, g1, g2, 0.5 * margin, &depth, dir, pos, wl);
+        double dist = margin - depth;
+        if (hit && dist >= margin) hit = false;
+        if (wl == 0) {
+          double* c = con + slot * L.cstride;
+          if (hit) { c[C_DIST] = dist; v3copy(c + C_POS, pos); v3copy(c + C_FRAME, dir); }
+          cpair[slot] = hit ? p : -1;
+        }
+      }
+      gsync();
+      const int nslots = ncon + k - k0;
+      // every thread counts the hits first (read-only), THEN warp 0 alone compacts in place: record j moves down to the next free slot
+      // (never overtakes an unread record).  (r02d: a version in which all threads walked the flags while warp 0 was already moving
+      // records let a slow thread read a flag that had just been overwritten - its contact count then differed from the others';
+      // found by racecheck once the workspace was in shared memory.)
+      int nhit = 0;
+      for (int j = ncon; j < nslots; j++) nhit += cpair[j] >= 0;
+      gsync();
+      if (wid == 0) {
+        int o2 = ncon;
+        for (int j = ncon; j < nslots; j++) {
+          const int p = cpair[j];
+          __syncwarp();  // every lane has read flag j before lane 0 may overwrite a lower slot
+          if (p < 0) continue;
+          if (o2 != j) {
+            for (int q = wl; q < C_FRAME + 3; q += 32) con[o2 * L.cstride + q] = con[j * L.cstride + q];
+            if (wl == 0) cpair[o2] = p;
+          }
+          o2++;
+        }
+      }
 #ifdef GE_DIAG
-    dg_k = k; dg_nhit = nhit; dg_nslots = nslots;
+      dg_k = k; dg_nhit = nhit; dg_nslots = nslots;
 #endif
+      ncon += nhit;
+      gsync();
+      if (ci >= ncand) break;
+    }
     if (overflow) *status |= 1;
-    ncon = out;
-    gsync();
+    nmpr = k;
   }
 #endif
   // ---- per-contact frame and solver parameters
@@ -935,7 +965,7 @@ __device__ __noinline__ int stage_collision(double* ws, int* wi, int lane, int* 
   }
   if (group_any(bad_pair)) *status |= 64;  // (every thread keeps its own copy of the status word: the flag has to be set by all of them)
   gsync();
-  return ncon;
+  return CollisionCounts{ncon, nsurv, nmpr};
 }
 
 }  // namespace ge

@@ -12,7 +12,7 @@ namespace ge {
 #define CTL_KP 16
 #define CTL_CTRL 24
 
-struct StepInfo { int ncon, nsr, niter; };
+struct StepInfo { int ncon, nsr, niter, ncand, nmpr; };  // ncand, nmpr: see CollisionCounts
 
 // Stage barriers: when GE_STAGE_SYNC is on, all warps of the CTA (one env each) enter collision, the constraint solver and the
 // integrator together, so that the SM's instruction cache serves the (large) stage code once per CTA instead of once per warp.
@@ -48,7 +48,10 @@ __device__ __noinline__ StepInfo forward(double* ws, int* wi, int lane, int* sta
   stage_fk(ws, lane);
   if (dbg) { nan_probe(ws + L.gmat, 9 * m.ngeom, lane, status, 9); nan_probe(ws + L.cdof, 6 * m.nv, lane, status, 9); }
   stage_barrier(sync);
-  si.ncon = stage_collision(ws, wi, lane, status);  // needs the geom frames only; bias forces / mass matrix reuse their storage
+  {
+    const CollisionCounts cc = stage_collision(ws, wi, lane, status);  // needs the geom frames only; bias forces / mass matrix reuse their storage
+    si.ncon = cc.ncon; si.ncand = cc.ncand; si.nmpr = cc.nmpr;
+  }
   if (dbg) nan_probe(ws + L.con, si.ncon * L.cstride < 16 * si.ncon ? 0 : 16 * 0 + si.ncon * 0, lane, status, 10);
   stage_rne(ws, lane);  // qfrc_smooth := bias
   stage_crb(ws, lane);

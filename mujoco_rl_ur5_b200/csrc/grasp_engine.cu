@@ -250,6 +250,32 @@ __global__ void __launch_bounds__(GE_LANES) k_debug(EnvArrays E, int env, int fi
     } else if (field == 9) { n = 1; if (lane == 0) out[0] = si.ncon; }
     else if (field == 10) { n = 1; if (lane == 0) out[0] = si.niter; }
     else if (field == 11) { n = 1; if (lane == 0) out[0] = si.nsr; }
+    else if (field == 12) { n = 1; if (lane == 0) out[0] = status; }
+    else if (field == 13) { n = 1; if (lane == 0) out[0] = si.ncand; }
+    else if (field == 14) { n = 1; if (lane == 0) out[0] = si.nmpr; }
+    else if (field == 15 && si.niter > 0) {  // layout of the last Newton Hessian build (none when the solve had no constraint rows)
+      // [hflag, total block doubles, ntree, then per tree: coupled, island label, owner warp, block offset, block rows]
+      const int *tcoupled = wi + L.i_tcoupled, *tlist = wi + L.i_tlist, *island = wi + L.i_island;
+      n = 3 + 5 * m.ntree;
+      if (lane == 0) {
+        int tot = 0;
+        for (int u = 0; u < m.ntree; u++) {
+          int r;
+          if (!tcoupled[u]) r = m.tree_dofnum[u];
+          else if (island[u] == u) r = tlist[u * GE_TLIST];
+          else continue;
+          tot += r * (r + 1) / 2;
+        }
+        out[0] = GE_NW > 1 ? wi[L.i_hflag] : 0; out[1] = tot; out[2] = m.ntree;
+      }
+      LANE_LOOP(t, (n <= cap ? m.ntree : 0)) {
+        const bool c = tcoupled[t] != 0;
+        double* o = out + 3 + 5 * t;
+        o[0] = c; o[1] = c ? island[t] : t;
+        o[2] = c && GE_NW > 1 ? tlist[island[t] * GE_TLIST + 1] : -1;  // owner warp (CTA-per-env build)
+        o[3] = T_HOFF(tlist, t); o[4] = c ? tlist[island[t] * GE_TLIST] : m.tree_dofnum[t];
+      }
+    }
   }
   if (lane == 0) *nout = n;
 }
@@ -687,6 +713,7 @@ extern "C" int ge_size(ge_handle h, int what) {
   switch (what) {
     case 0: return h->hm.nq; case 1: return h->hm.nv; case 2: return h->hm.nbody; case 3: return h->hm.ngeom; case 4: return h->hm.nu;
     case 5: return h->n_envs; case 6: return h->lay.maxcon; case 7: return h->lay.total_bytes; case 8: return h->wpb; case 9: return h->lay.ws_global;
+    case 10: return h->lay.hcap; case 11: return h->lay.hfull;
   }
   return GE_ERR_ARG;
 }
@@ -896,9 +923,10 @@ extern "C" int ge_render(ge_handle h, int cam, int width, int height, uint8_t* r
 extern "C" int ge_debug_forward(ge_handle h, int env, const char* field, double* out, int cap) {
   if (!h || !field || !out || env < 0 || env >= h->n_envs) return fail(GE_ERR_ARG, "ge_debug_forward: bad argument");
   if (bind(h)) return GE_ERR_CUDA;
-  static const char* names[] = {"xpos", "xmat", "cdof", "qM", "qfrc_bias", "qacc_smooth", "qacc", "qfrc_constraint", "contact", "ncon", "niter", "nsr"};
+  static const char* names[] = {"xpos", "xmat", "cdof", "qM", "qfrc_bias", "qacc_smooth", "qacc", "qfrc_constraint", "contact", "ncon", "niter", "nsr",
+                                "status", "ncand", "nmpr", "hlayout"};
   int f = -1;
-  for (int i = 0; i < 12; i++) if (!strcmp(names[i], field)) f = i;
+  for (int i = 0; i < (int)(sizeof names / sizeof names[0]); i++) if (!strcmp(names[i], field)) f = i;
   if (f < 0) return fail(GE_ERR_ARG, "ge_debug_forward: unknown field %s", field);
   if (cap > (1 << 16)) cap = 1 << 16;
   k_debug<<<1, GE_LANES, h->ws_smem, h->stream>>>(h->E, env, f, h->d_dbg, cap, h->d_nout);

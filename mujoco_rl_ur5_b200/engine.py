@@ -96,7 +96,8 @@ class BatchedEngine:
 
     def size(self, what):
         """ge_size: 0 nq, 1 nv, 2 nbody, 3 ngeom, 4 nu, 5 n_envs, 6 max contacts, 7 workspace bytes per env, 8 envs per CTA,
-        9 workspace placement (0 shared memory, 1 HBM rows)"""
+        9 workspace placement (0 shared memory, 1 HBM rows), 10 doubles of the Newton Hessian block region in the workspace (hcap),
+        11 doubles of a full packed Hessian = of one env's HBM overflow row (hfull)"""
         return int(self.L.ge_size(self.h, int(what)))
 
     # ------------------------------------------------------------------ helpers
@@ -291,6 +292,8 @@ class BatchedEngine:
 
     # ------------------------------------------------------------------ diagnostics
     def debug_forward(self, env, field, cap=1 << 16):
+        """ge_debug_forward: one forward pass of env `env` on its current state, one internal field copied out (names and layouts in
+        include/grasp_engine.h; "status", "ncand", "nmpr" and "hlayout" describe the contact list and the last Newton Hessian build)"""
         buf = (C.c_double * cap)()
         n = self._ck(self.L.ge_debug_forward(self.h, int(env), field.encode(), buf, cap), "ge_debug_forward")
         return np.array(buf[:n], dtype=np.float64)

@@ -102,11 +102,12 @@ typedef struct {
   /* dynamics */
   double *qM, *qLD, *qH, *qfrc_bias, *qfrc_passive, *qfrc_actuator, *qfrc_smooth, *qacc_smooth, *qfrc_constraint, *qacc;
   /* contacts + constraints */
-  int ncon, nefc, ne, nl, nefc_max;
+  int ncon, nefc, ne, nl, nefc_max, maxcon; /* maxcon: contacts kept (<= MAXCON, orc_set_maxcon), later ones set con_overflow */
   Contact con[MAXCON];
   double *efc_J, *efc_B, *efc_pos, *efc_margin, *efc_diag, *efc_R, *efc_aref, *efc_force, *efc_AR;
   int* efc_type;
   int solver_iter, con_overflow, solver; /* solver: 0 = Newton (MuJoCo default, what the MJCF implies), 1 = PGS */
+  int ncand;                             /* pairs that passed the broad phase in the last collision stage */
   double *tmp1, *tmp2, *nt_H, *nt_grad, *nt_search, *nt_Ma, *nt_Mv, *nt_jar, *nt_jv;
   int* nt_active;
 } Env;
@@ -190,6 +191,7 @@ Env* orc_env_create(Model* m) {
   e->qfrc_bias = DALLOC(nv); e->qfrc_passive = DALLOC(nv); e->qfrc_actuator = DALLOC(nv); e->qfrc_smooth = DALLOC(nv);
   e->qacc_smooth = DALLOC(nv); e->qfrc_constraint = DALLOC(nv); e->qacc = DALLOC(nv);
   e->nefc_max = m->neq + m->njnt + 10 * MAXCON;
+  e->maxcon = MAXCON;
   e->efc_J = DALLOC((size_t)e->nefc_max * nv); e->efc_B = DALLOC((size_t)e->nefc_max * nv);
   e->efc_pos = DALLOC(e->nefc_max); e->efc_margin = DALLOC(e->nefc_max); e->efc_diag = DALLOC(e->nefc_max);
   e->efc_R = DALLOC(e->nefc_max); e->efc_aref = DALLOC(e->nefc_max); e->efc_force = DALLOC(e->nefc_max); e->efc_AR = DALLOC(e->nefc_max);
@@ -414,7 +416,7 @@ static void make_frame(double* fr) { /* fr[0..2] = unit normal given; fill two t
 }
 static void add_contact(Env* e, int pair, double dist, const double* pos, const double* normal) {
   const Model* m = e->m;
-  if (e->ncon >= MAXCON) { e->con_overflow = 1; return; }
+  if (e->ncon >= e->maxcon) { e->con_overflow = 1; return; }
   Contact* c = &e->con[e->ncon++];
   c->dist = dist; v3copy(c->pos, pos); v3copy(c->frame, normal); make_frame(c->frame);
   c->margin = m->pair_margin[pair]; c->dim = m->pair_condim[pair];
@@ -893,7 +895,7 @@ static int pair_is_analytic(int t1, int t2) {
  * (Contact order only affects floating-point summation order in the solver; the CUDA engine emits the same order.) */
 static void collision(Env* e) {
   const Model* m = e->m;
-  e->ncon = 0; e->con_overflow = 0;
+  e->ncon = 0; e->con_overflow = 0; e->ncand = 0;
   for (int pass = 0; pass < 2; pass++)
   for (int p = 0; p < m->npair; p++) {
     int g1 = m->pair_geom[2 * p], g2 = m->pair_geom[2 * p + 1], t1 = m->geom_type[g1], t2 = m->geom_type[g2];
@@ -904,6 +906,7 @@ static void collision(Env* e) {
       double n[3], d[3];
       m3col(n, e->gmat + 9 * g1, 2); v3sub(d, c2, e->gpos + 3 * g1);
       if (v3dot(d, n) > m->geom_rbound[g2] + margin) continue;
+      e->ncand++;
       if (t2 == G_SPHERE) col_plane_sphere(e, p, g1, g2);
       else if (t2 == G_BOX) col_plane_box(e, p, g1, g2);
       else if (t2 == G_MESH) col_plane_mesh(e, p, g1, g2);
@@ -918,6 +921,7 @@ static void collision(Env* e) {
     if (v3dot(d, d) > rs * rs) continue;
     if (!(t1 == G_SPHERE && t2 == G_SPHERE) &&
         obb_separated(c1, e->gmat + 9 * g1, m->geom_obbhalf + 3 * g1, c2, e->gmat + 9 * g2, m->geom_obbhalf + 3 * g2, margin)) continue;
+    e->ncand++;
     if (t1 == G_SPHERE && t2 == G_SPHERE) col_sphere_sphere(e, p, g1, g2);
     else if (t1 == G_SPHERE && t2 == G_BOX) col_sphere_box(e, p, g1, g2);
     else if (t1 == G_BOX && t2 == G_BOX) col_box_box(e, p, g1, g2);
@@ -1608,6 +1612,13 @@ double* orc_last_input(Env* e) { return e->last_input; }
 long orc_substeps(Env* e) { return e->substeps; }
 void orc_set_dt_pid(Env* e, double dt) { e->dt_pid = dt; }
 void orc_set_solver(Env* e, int solver) { e->solver = solver; }
+/* contact capacity: the list keeps the first n contacts of its emission order (analytic pairs, then MPR pairs, both in pair order),
+ * like the CUDA engine's list of `maxcon` contacts; clamped to [0, MAXCON] */
+void orc_set_maxcon(Env* e, int n) { e->maxcon = n < 0 ? 0 : (n > MAXCON ? MAXCON : n); }
+/* 1 if the last collision stage found more contacts than the capacity */
+int orc_con_overflow(Env* e) { return e->con_overflow; }
+/* broad-phase survivors of the last collision stage (the engine's "ncand") */
+int orc_ncand(Env* e) { return e->ncand; }
 /* set_state + controller re-sync as GraspEnv.reset_model does (GraspingEnv.py:466-470) */
 void orc_reset(Env* e, const double* qpos, const double* qvel) {
   const Model* m = e->m;

@@ -43,6 +43,9 @@ def lib():
         L.orc_substeps.argtypes = [P]
         L.orc_set_dt_pid.argtypes = [P, C.c_double]
         L.orc_set_solver.argtypes = [P, C.c_int]
+        L.orc_set_maxcon.argtypes = [P, C.c_int]
+        L.orc_con_overflow.argtypes = [P]
+        L.orc_ncand.argtypes = [P]
         L.orc_reset.argtypes = [P, D, D]
         L.orc_field.restype = D
         L.orc_field.argtypes = [P, C.c_char_p, I]
@@ -137,6 +140,21 @@ class OracleEnv:
 
     def set_solver(self, name):
         self.L.orc_set_solver(self.env, {"newton": 0, "pgs": 1}[name])
+
+    def set_maxcon(self, n):
+        """contact capacity (default 256): later contacts of the emission order (analytic pairs, then MPR pairs, both in pair
+        order) are dropped and `con_overflow` is set, as in the CUDA engine's list of GE_MAXCON contacts"""
+        self.L.orc_set_maxcon(self.env, int(n))
+
+    @property
+    def con_overflow(self):
+        """1 if the last collision stage found more contacts than the capacity"""
+        return int(self.L.orc_con_overflow(self.env))
+
+    @property
+    def ncand(self):
+        """pairs that passed the broad phase in the last collision stage"""
+        return int(self.L.orc_ncand(self.env))
 
     def forward(self):
         self.L.orc_forward(self.env)

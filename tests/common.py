@@ -27,6 +27,17 @@ def object_positions(A, qpos):
     return np.array([qpos[8 + 7 * i:11 + 7 * i] + A["body_pos"][first + i] for i in range(nobj)])
 
 
+def contact_is_analytic(A, contacts):
+    """per contact row (geom ids in columns 13, 14): True if its pair has a closed-form narrow phase, False if it goes through MPR
+    (the oracle's and the engine's pair_is_analytic; geom types 0 plane, 2 sphere, 3 capsule, 5 cylinder, 6 box, 7 mesh)"""
+    gtype = np.asarray(A["geom_type"]).ravel()
+    out = []
+    for g1, g2 in np.asarray(contacts)[:, 13:15].astype(int):
+        t1, t2 = int(gtype[g1]), int(gtype[g2])
+        out.append(t1 == 0 or (t1 == 2 and t2 in (2, 3, 5, 6)) or (t1, t2) in ((6, 6), (3, 3)))
+    return np.array(out, bool)
+
+
 def reset_qpos_scene_b(A, env_index):
     """Scene-B reset = the live rule of GraspingEnv.py:418-430 (x, y, z, then Quaternion.random()'s three uniforms per object),
     RNG = RandomState(20000 + env_index)."""

@@ -4,7 +4,7 @@ and a settle run (objects end up resting on the table or the floor, contacts con
 import numpy as np
 import pytest
 
-from tests.common import HOME, reset_qpos_scene_b
+from tests.common import HOME, contact_is_analytic, reset_qpos_scene_b
 
 S2 = np.sqrt(0.5)
 
@@ -114,3 +114,37 @@ def test_objects_fall_and_come_to_rest(orcb, scene_b):
     orcb.reset(q0)
     orcb.move_group("All", HOME + 0.05, 1e-9, 599)
     assert np.array_equal(q1, orcb.qpos)  # deterministic
+
+
+def test_contact_capacity_keeps_a_prefix_of_the_emission_order(scene_b):
+    """set_maxcon(n): the list is the first n contacts of the uncapped list (analytic pairs, then MPR pairs), the overflow flag is
+    set iff the uncapped count exceeds n, and the default capacity gives the same results as before any cap was set"""
+    from oracle.oracle_py import OracleEnv
+
+    blob, A, _ = scene_b
+    o = OracleEnv(blob)
+    o.reset(reset_qpos_scene_b(A, 3))
+    o.move_group("All", HOME + 0.05, 1e-9, 399)
+    q, v = o.qpos.copy(), o.qvel.copy()
+    o.reset(q, v)
+    o.forward()
+    full, total = o.contacts(), o.ncon
+    acc, frc = o.field("qacc"), o.field("qfrc_constraint")
+    assert total >= 25 and o.con_overflow == 0
+    analytic = contact_is_analytic(A, full)
+    n_analytic = int(analytic.sum())
+    assert 0 < n_analytic < total and analytic[:n_analytic].all()  # analytic contacts first, then the MPR ones
+    for cap in (total + 5, total, total - 1, n_analytic + (total - n_analytic) // 2, n_analytic, 16, 0):
+        o.set_maxcon(cap)
+        o.reset(q, v)
+        o.forward()
+        assert o.ncon == min(cap, total), cap
+        assert np.array_equal(o.contacts(), full[:min(cap, total)]), cap
+        assert o.con_overflow == int(total > cap), cap
+        assert np.isfinite(o.field("qacc")).all()
+    o.set_maxcon(256)
+    o.reset(q, v)
+    o.forward()
+    assert o.ncon == total and o.con_overflow == 0
+    assert np.array_equal(o.field("qacc"), acc) and np.array_equal(o.field("qfrc_constraint"), frc)
+    o.close()

@@ -83,7 +83,7 @@ __device__ __noinline__ void build_hessian(double* ws, int* wi, int ncon, int ns
   LANE_LOOP(t, m.ntree) {
     int cnt = 0;
     if (!tcoupled[t]) {
-      for (int ci = 0; ci < ncon; ci++)
+      NO_UNROLL for (int ci = 0; ci < ncon; ci++)
         if (wi[L.i_cact + ci] && (wi[L.i_ct1 + ci] == t || wi[L.i_ct2 + ci] == t)) { if (cnt < GE_TCAP) tlist[t * GE_TLIST + cnt] = ci; cnt++; }
       if (cnt > GE_TCAP) { tcoupled[t] = 1; cnt = 0; }  // too many contacts for the list: this tree takes the coupled path
     }
@@ -188,9 +188,9 @@ __device__ __noinline__ void build_hessian(double* ws, int* wi, int ncon, int ns
     const int t = m.dof_treeindex[i], lo = m.tree_dofadr[t];
     const int r0 = tcoupled[t] ? tcount[t] : 0, r = r0 + i - lo;
     double* row = H + T_HOFF(tlist, t) + r * (r + 1) / 2;
-    for (int j = 0; j <= r; j++) row[j] = 0;
+    NO_UNROLL for (int j = 0; j <= r; j++) row[j] = 0;
     int a = m.dof_Madr[i], k = 0;
-    for (int j = i; j >= 0; j = m.dof_parentid[j], k++) row[r0 + j - lo] = qM[a + k];
+    NO_UNROLL for (int j = i; j >= 0; j = m.dof_parentid[j], k++) row[r0 + j - lo] = qM[a + k];
   }
   gsync();
   // ---- uncoupled trees: one 8-lane group per tree, GE_LANES / 8 trees at a time, every group walking ITS OWN contact list so that
@@ -207,7 +207,7 @@ __device__ __noinline__ void build_hessian(double* ws, int* wi, int ncon, int ns
       int maxcnt = cnt;
 #pragma unroll
       for (int o = 16; o > 0; o >>= 1) maxcnt = max(maxcnt, __shfl_xor_sync(FULL, maxcnt, o));
-      for (int n = 0; n < maxcnt; n++) {
+      NO_UNROLL for (int n = 0; n < maxcnt; n++) {
         const bool act = n < cnt && l < nt;
         double J[6] = {0, 0, 0, 0, 0, 0}, tw[6] = {0, 0, 0, 0, 0, 0};
         if (act) {
@@ -222,7 +222,7 @@ __device__ __noinline__ void build_hessian(double* ws, int* wi, int ncon, int ns
         }
         for (int f = 0; f < GE_GROUP; f++) {
           double h = 0;
-          for (int k = 0; k < m.maxdim; k++) h += tw[k] * __shfl_sync(FULL, J[k], gw + f);
+          NO_UNROLL for (int k = 0; k < m.maxdim; k++) h += tw[k] * __shfl_sync(FULL, J[k], gw + f);
           if (act && l >= f && f < nt && h != 0.0) Hb[HIDX(l, f)] += h;
         }
       }
@@ -247,7 +247,7 @@ __device__ __noinline__ void build_hessian(double* ws, int* wi, int ncon, int ns
   if (!any_coupled) return;
   // ---- coupled trees: warp-cooperative accumulation, one lane per dof of the contact; a contact belongs to the warp that owns its
   // island.  Block-local row of dof d of tree t: tcount[t] + d - tree_dofadr[t].
-  for (int ci = 0; ci < ncon; ci++) {
+  NO_UNROLL for (int ci = 0; ci < ncon; ci++) {
     int mask = wi[L.i_cact + ci];
     if (!mask) continue;
     int b1 = wi[L.i_cb1 + ci], b2 = wi[L.i_cb2 + ci], t1 = wi[L.i_ct1 + ci], t2 = wi[L.i_ct2 + ci];
@@ -281,7 +281,7 @@ __device__ __noinline__ void build_hessian(double* ws, int* wi, int ncon, int ns
       const int tt = m.dof_treeindex[mydof];
       myrow = tcount[tt] + mydof - m.tree_dofadr[tt];
     }
-    for (int j0 = 0; j0 < n; j0 += P) {
+    NO_UNROLL for (int j0 = 0; j0 < n; j0 += P) {
       const int j = j0 + p_;
       const bool v = act && j < n;
       const int src = v ? j : 0;  // lane j (p = 0) holds row j

@@ -9,6 +9,7 @@
 #pragma once
 #include "ge_math.cuh"
 #include "ge_model.cuh"
+#include "ge_clocks.cuh"
 
 namespace ge {
 
@@ -17,7 +18,9 @@ __constant__ Layout c_L;
 __shared__ double* g_hovf;    // CTA-per-env build: HBM overflow row for the Hessian blocks of the env this CTA holds (may be null)
 __constant__ int c_nancheck;  // GE_NANCHECK=1: record in status bits 8.. the first pipeline stage that produced a non-finite value
 
-#define LANE_LOOP(i, n) for (int i = lane; i < (n); i += GE_LANES)
+// Trip counts are data (items per lane, mostly 1 or 2): unrolling them only multiplies the code every warp has to fetch.
+#define LANE_LOOP(i, n) _Pragma("unroll 1") for (int i = lane; i < (n); i += GE_LANES)
+#define NO_UNROLL _Pragma("unroll 1")
 
 // ------------------------------------------------------------------------------------------------ kinematics
 // Three lane-parallel phases, no level synchronisation: (1) every body's transform relative to its parent,
@@ -821,6 +824,7 @@ __device__ __noinline__ CollisionCounts stage_collision(double* ws, int* wi, int
 #endif
   if (ncon > L.maxcon) { ncon = L.maxcon; *status |= 1; }
   gsync();
+  GE_CLK(SC_COLLISION);
   // ---- convex pairs through MPR
   int nmpr = 0;
 #if GE_NW == 1
@@ -923,6 +927,7 @@ __device__ __noinline__ CollisionCounts stage_collision(double* ws, int* wi, int
     nmpr = k;
   }
 #endif
+  GE_CLK(SC_MPR);
   // ---- per-contact frame and solver parameters
   bool bad_pair = false;
   LANE_LOOP(i, ncon) {

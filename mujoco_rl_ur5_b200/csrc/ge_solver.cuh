@@ -191,7 +191,7 @@ __device__ __noinline__ double nt_update(double* ws, int* wi, int ncon, int nsr,
   LANE_LOOP(b, m.nbody) {
     double w[6] = {0, 0, 0, 0, 0, 0};
     if (m.body_lastdof[b] >= 0)
-      for (int i = 0; i < ncon; i++) {
+      NO_UNROLL for (int i = 0; i < ncon; i++) {
         int b1 = wi[L.i_cb1 + i], b2 = wi[L.i_cb2 + i];
         if (b2 == b) for (int k = 0; k < 6; k++) w[k] += Wc[6 * i + k];
         if (b1 == b) for (int k = 0; k < 6; k++) w[k] -= Wc[6 * i + k];
@@ -202,7 +202,7 @@ __device__ __noinline__ double nt_update(double* ws, int* wi, int ncon, int nsr,
   LANE_LOOP(b, m.nbody) {
     double s[6] = {0, 0, 0, 0, 0, 0};
     int n = m.body_subtreenum[b];
-    for (int c2 = b; c2 < b + n; c2++) for (int k = 0; k < 6; k++) s[k] += Wb[6 * c2 + k];
+    NO_UNROLL for (int c2 = b; c2 < b + n; c2++) for (int k = 0; k < 6; k++) s[k] += Wb[6 * c2 + k];
     for (int k = 0; k < 6; k++) Wsub[6 * b + k] = s[k];
   }
   gsync();
@@ -210,7 +210,7 @@ __device__ __noinline__ double nt_update(double* ws, int* wi, int ncon, int nsr,
   const double* cdof = ws + L.cdof;
   LANE_LOOP(d, m.nv) {
     double s = dot6(cdof + 6 * d, Wsub + 6 * m.dof_bodyid[d]);
-    for (int i = 0; i < nsr; i++) {
+    NO_UNROLL for (int i = 0; i < nsr; i++) {
       double f = srv(ws, SR_JV, i);
       if (wi[L.i_srA + i] == d) s += srv(ws, SR_CA, i) * f;
       if (wi[L.i_srB + i] == d) s += srv(ws, SR_CB, i) * f;
@@ -275,34 +275,45 @@ __device__ __noinline__ int solve_newton(double* ws, int* wi, int lane, int ncon
     LANE_LOOP(i, nsr) srv(ws, SR_JA, i) = srv(ws, SR_JV, i);
   }
   gsync();
+  GE_CLK(SC_NEWTON);
   mul_M(qM, Ma, qacc, lane);
+  GE_CLK(SC_MULM_COLD);
+  GE_WARM(SC_MULM_COLD, SC_WARM_MULM, mul_M(qM, Ma, qacc, lane));
   double cost_c = nt_update(ws, wi, ncon, nsr, lane), gauss = 0;
+  GE_CLK(SC_NT_UPDATE);
   LANE_LOOP(d, nv) gauss += 0.5 * (Ma[d] - qfrc_smooth[d]) * (qacc[d] - qacc_smooth[d]);
   double cost = group_sum(gauss) + cost_c;
   double scale = 1.0 / (m.meaninertia * (nv > 1 ? nv : 1));
   int niter = 0;
-  for (int it = 0; it < m.iterations; it++) {
+  NO_UNROLL for (int it = 0; it < m.iterations; it++) {
     double gn = 0;
     LANE_LOOP(d, nv) { double g = Ma[d] - qfrc_smooth[d] - qfc[d]; grad[d] = g; gn += g * g; }
     gn = group_sum(gn);
     gsync();
     if (it > 0 && scale * sqrt(gn) < m.tolerance) break;
+    GE_CLK(SC_NEWTON);
     if (it == 0) newton_barrier(sync);
+    GE_CLK(SC_BARRIER);
     build_hessian(ws, wi, ncon, nsr, lane);
+    GE_CLK(SC_HESSIAN);
     if (it == 0) newton_barrier(sync);
+    GE_CLK(SC_BARRIER);
     cholesky_solve(ws, wi, search, grad, lane);
+    GE_CLK(SC_CHOL);
     mul_M(qM, Mv, search, lane);
     double g1 = 0, g2 = 0, sn = 0;
     LANE_LOOP(d, nv) { g1 += search[d] * (Ma[d] - qfrc_smooth[d]); g2 += 0.5 * search[d] * Mv[d]; sn += search[d] * search[d]; }
     g1 = group_sum(g1); g2 = group_sum(g2); sn = sqrt(group_sum(sn));
     body_vel(ws, search, lane); contact_base(ws, wi, ncon, jv, lane); simple_base(ws, wi, nsr, search, SR_JV, lane);
     gsync();
+    GE_CLK(SC_NEWTON);
     if (it == 0) newton_barrier(sync);
+    GE_CLK(SC_BARRIER);
     // exact line search: safeguarded 1-D Newton on the convex piecewise-quadratic cost along `search`
     double gtol = m.tolerance * 0.01 * sn * m.meaninertia * (nv > 1 ? nv : 1);
     if (gtol < GE_MINVAL) gtol = GE_MINVAL;
     double alpha = 0, lo = 0, hi = -1;
-    for (int ls = 0; ls < 50; ls++) {
+    NO_UNROLL for (int ls = 0; ls < 50; ls++) {
       double d1 = 0, d2 = 0;
       LANE_LOOP(i, ncon) {
         const double* c = ws + L.con + i * L.cstride;
@@ -326,7 +337,9 @@ __device__ __noinline__ int solve_newton(double* ws, int* wi, int lane, int ncon
       if (hi >= 0 && (next <= lo || next >= hi)) next = 0.5 * (lo + hi);
       alpha = next;
     }
+    GE_CLK(SC_LINESEARCH);
     if (it == 0) newton_barrier(sync);
+    GE_CLK(SC_BARRIER);
     niter = it + 1;
     if (alpha == 0) break;
     LANE_LOOP(d, nv) { qacc[d] += alpha * search[d]; Ma[d] += alpha * Mv[d]; }
@@ -334,7 +347,9 @@ __device__ __noinline__ int solve_newton(double* ws, int* wi, int lane, int ncon
     LANE_LOOP(i, nsr) srv(ws, SR_JA, i) += alpha * srv(ws, SR_JV, i);
     gsync();
     double oldcost = cost;
+    GE_CLK(SC_NEWTON);
     cost_c = nt_update(ws, wi, ncon, nsr, lane);
+    GE_CLK(SC_NT_UPDATE);
     gauss = 0;
     LANE_LOOP(d, nv) gauss += 0.5 * (Ma[d] - qfrc_smooth[d]) * (qacc[d] - qacc_smooth[d]);
     cost = group_sum(gauss) + cost_c;

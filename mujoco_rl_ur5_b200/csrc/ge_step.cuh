@@ -46,15 +46,21 @@ __device__ __noinline__ StepInfo forward(double* ws, int* wi, int lane, int* sta
   const bool dbg = c_nancheck != 0;
   if (dbg) { nan_probe(ws + L.qpos, m.nq, lane, status, 8); nan_probe(ws + L.qvel, m.nv, lane, status, 8); nan_probe(ws + L.ctl, 32, lane, status, 8); }
   stage_fk(ws, lane);
+  GE_CLK(SC_FK);
+  GE_WARM(SC_FK, SC_WARM_FK, stage_fk(ws, lane));
   if (dbg) { nan_probe(ws + L.gmat, 9 * m.ngeom, lane, status, 9); nan_probe(ws + L.cdof, 6 * m.nv, lane, status, 9); }
   stage_barrier(sync);
+  GE_CLK(SC_BARRIER);
   {
     const CollisionCounts cc = stage_collision(ws, wi, lane, status);  // needs the geom frames only; bias forces / mass matrix reuse their storage
     si.ncon = cc.ncon; si.ncand = cc.ncand; si.nmpr = cc.nmpr;
   }
+  GE_CLK(SC_COLLISION);
   if (dbg) nan_probe(ws + L.con, si.ncon * L.cstride < 16 * si.ncon ? 0 : 16 * 0 + si.ncon * 0, lane, status, 10);
   stage_rne(ws, lane);  // qfrc_smooth := bias
   stage_crb(ws, lane);
+  GE_CLK(SC_RNE_CRB);
+  GE_WARM(SC_RNE_CRB, SC_WARM_RNE_CRB, stage_rne(ws, lane); stage_crb(ws, lane));
   if (dbg) { nan_probe(ws + L.qM, m.nM, lane, status, 11); nan_probe(ws + L.qfrc_smooth, m.nv, lane, status, 11); }
   // smooth forces: passive (joint damping) - bias + actuation (torque motors, gear * clamp(ctrl))
   const double *qvel = ws + L.qvel, *ctrl = ws + L.ctl + CTL_CTRL;
@@ -78,14 +84,18 @@ __device__ __noinline__ StepInfo forward(double* ws, int* wi, int lane, int* sta
     solve_trees(ws + L.qLD, qas, lane);
   }
   if (dbg) nan_probe(qas, m.nv, lane, status, 12);
+  GE_CLK(SC_MASS);
   stage_barrier(sync);
+  GE_CLK(SC_BARRIER);
   si.nsr = stage_constraints(ws, wi, lane, si.ncon, status);
+  GE_CLK(SC_CONSTRAINTS);
   if (dbg) nan_probe(ws + L.sr, 6 * GE_MAXSR * 0 + 4 * 0, lane, status, 13);
   si.niter = solve_newton(ws, wi, lane, si.ncon, si.nsr, GE_STAGE_SYNC && sync);
   if (dbg) nan_probe(ws + L.qacc, m.nv, lane, status, 14);
   if (si.niter >= m.iterations) *status |= 4;
   LANE_LOOP(d, m.nv) ws[L.qaccws + d] = ws[L.qacc + d];
   gsync();
+  GE_CLK(SC_NEWTON);
   return si;
 }
 
@@ -94,6 +104,7 @@ __device__ __noinline__ StepInfo sim_step(double* ws, int* wi, int lane, int* st
   const DevModel& m = c_m; const Layout& L = c_L;
   StepInfo si = forward(ws, wi, lane, status, sync);
   stage_barrier(sync);
+  GE_CLK(SC_BARRIER);
   double h = m.timestep;
   double *acc = ws + L.grad, *qH = ws + L.qLD, *qvel = ws + L.qvel, *qpos = ws + L.qpos;
   LANE_LOOP(d, m.nv) acc[d] = ws[L.qfrc_smooth + d] + ws[L.qfrc_constraint + d];
@@ -125,6 +136,8 @@ __device__ __noinline__ StepInfo sim_step(double* ws, int* wi, int lane, int* st
   }
   if (group_any(bad)) *status |= 2;
   gsync();
+  GE_CLK(SC_EULER);
+  GE_CLK_COUNT(SC_SUBSTEPS);
   return si;
 }
 

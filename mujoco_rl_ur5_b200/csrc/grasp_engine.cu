@@ -129,6 +129,7 @@ __global__ void GE_RUN_BOUNDS k_run(EnvArrays E, int n_env, int nsub, int quota,
   EnvRegs r;
   int env = -1, left = 0, visit_len = 0;
   bool exhausted = false, running = false;  // running: the group has a loaded visit of `env` in progress
+  GE_CLK_START();
   for (;;) {
     // ---- a group without an environment takes tasks until it finds a busy, unlocked environment (or the launch has none left)
     while (env < 0 && !exhausted) {
@@ -158,13 +159,15 @@ __global__ void GE_RUN_BOUNDS k_run(EnvArrays E, int n_env, int nsub, int quota,
       left = visit_len = nsub - d < quota ? nsub - d : quota;
       running = true;
     }
+    GE_CLK(SC_SCHED);
 #if GE_NW == 1
     __syncwarp();
     if (!__syncthreads_or(env >= 0)) break;  // all warps (= envs) of the CTA are out of work
 #else
     if (env < 0) break;                      // one env per CTA: `env` is the same in every thread
 #endif
-    if (env < 0) { stage_barriers_idle((stage_sync & 1) != 0); continue; }
+    GE_CLK(SC_BARRIER);
+    if (env < 0) { stage_barriers_idle((stage_sync & 1) != 0); GE_CLK(SC_BARRIER); continue; }
     bool stepped = false;
     // one iteration of the reference loop that ends in a physics step (or the env going idle)
     while (true) {
@@ -172,7 +175,9 @@ __global__ void GE_RUN_BOUNDS k_run(EnvArrays E, int n_env, int nsub, int quota,
         if (r.p.phase == PH_NONE || !prog_advance(r.p, r.c, ws, lane, base, r.info, &r.reward)) { running = false; break; }
         continue;
       }
+      GE_CLK(SC_SCHED);
       double delta = pid_and_delta(ws, lane, r.c.mask, c_m.timestep);
+      GE_CLK(SC_PID);
       if (delta < r.c.tol) { r.c.result = 1; r.c.reached = 1; }
       if (r.c.steps > r.c.maxsteps) { r.c.result = 2; r.c.active = 0; continue; }
       if (!(stage_sync & 0x100)) sim_step(ws, wi, lane, &r.status, (stage_sync & 1) != 0);  // bit 8: GE_DBG_NOSTEP (scheduler-only experiments)
@@ -181,7 +186,7 @@ __global__ void GE_RUN_BOUNDS k_run(EnvArrays E, int n_env, int nsub, int quota,
       if (r.c.reached) r.c.active = 0;
       break;
     }
-    if (!stepped) stage_barriers_idle((stage_sync & 1) != 0);
+    if (!stepped) { GE_CLK(SC_SCHED); stage_barriers_idle((stage_sync & 1) != 0); GE_CLK(SC_BARRIER); }
     if (--left <= 0 || !running) {
       // a movement that just ended inside the last iteration still has to hand over to the program (no sub-step involved)
       while (!r.c.active && r.p.phase != PH_NONE) { if (!prog_advance(r.p, r.c, ws, lane, base, r.info, &r.reward)) break; }
@@ -202,6 +207,8 @@ __global__ void GE_RUN_BOUNDS k_run(EnvArrays E, int n_env, int nsub, int quota,
       if (!again) env = -1;
     }
   }
+  GE_CLK(SC_SCHED);
+  GE_CLK_STOP();
 }
 // number of environments that still have a movement / program pending (ge_run's loop condition)
 __global__ void k_count_busy(EnvArrays E, int n_env) {
@@ -945,3 +952,19 @@ extern "C" int ge_counters(ge_handle h, int64_t* kernel_launches, int64_t* subst
   if (substep_launches) *substep_launches = h->substep_launches;
   return GE_OK;
 }
+
+#ifdef GE_STAGE_CLOCKS
+// profile builds only (ge_clocks.cuh): copies the per-warp-slot stage counters out, [GE_CLK_SLOTS][SC_NUM] u64, then zeroes them when
+// `reset` is set.  Exported under the variant's own name (ge_stage_clocks_smem / _hbm): the dispatcher does not know it.
+extern "C" int GE_API(ge_stage_clocks)(unsigned long long* out, int reset) {
+  CK(cudaDeviceSynchronize());
+  if (out) CK(cudaMemcpyFromSymbol(out, g_stage_clk, sizeof(g_stage_clk)));
+  if (reset) {
+    void* p = nullptr;
+    CK(cudaGetSymbolAddress(&p, g_stage_clk));
+    CK(cudaMemset(p, 0, sizeof(g_stage_clk)));
+    CK(cudaDeviceSynchronize());
+  }
+  return GE_OK;
+}
+#endif

@@ -73,6 +73,24 @@ int gq_obs_to_state(const unsigned char* rgb, const float* depth, float depth_th
 int gq_obs_to_state_train(const unsigned char* rgb, const float* depth, float depth_threshold, float noise_std, unsigned long long seed,
                           const long long* env_index, unsigned int step, const float* jitter, const int* order, float* scratch_red, float* state,
                           void* state_nhwc_bf16, int B, int HW, void* stream);
+/* The same training transform with every random choice keyed, for the online trainer and its observation replay.  Row b of the output
+ * is image slot[b] of rgb [S,HW,3] u8 / depth [S,HW] f32 (slot [B] int64, NULL: b), keyed on env_index[b] (int64, the global env id)
+ * and step[b] (uint32): the depth noise as in gq_obs_to_state_train, and the ColorJitter factors and operation order drawn from the
+ * same generator (the table in csrc/qnet.cu), so the state of a stored observation is regenerated bit for bit.
+ * Out: jitter_out [B,4] f32 and order_out [B,4] int32 = the drawn factors and order (what gq_obs_to_state_train would be given);
+ * state [B,4,HW] f32 and/or state_nhwc_bf16 [B,HW,4] bf16 (either may be NULL); scratch_red [B,4] f32. */
+int gq_obs_to_state_keyed(const unsigned char* rgb, const float* depth, const long long* slot, const long long* env_index, const unsigned int* step,
+                          float depth_threshold, float noise_std, unsigned long long seed, float* scratch_red, float* jitter_out, int* order_out,
+                          float* state, void* state_nhwc_bf16, int B, int HW, void* stream);
+/* Grasp_Agent.epsilon_greedy (Grasping_Agent_multidiscrete.py:232-282) for B envs.  depth [B,H,W] f32 (the current observation),
+ * greedy_idx [B] int32 (gq_argmax), eps [B] f64, env_index [B] int64 (global env ids), seed / step: key and counter of the keyed draws.
+ * Env b is greedy iff its uniform u > eps[b]; otherwise it takes the first of its candidates (flat rot*H*W + y*W + x) whose pixel lies
+ * on or above z_min in the world (TABLE_HEIGHT - 0.01), with pixel_2_world's arithmetic for the camera (fovy, cam_pos[3], cam_mat[9]:
+ * plain host doubles, the camera of the scene arrays).  After max_draws rejected candidates the last one is taken and exhausted[b] = 1.
+ * Out: action [B,2] int32 (pixel y*W + x, rotation), is_random [B] u8, exhausted [B] u8. */
+int gq_sample_actions(const float* depth, const int* greedy_idx, const double* eps, unsigned long long seed, const long long* env_index, unsigned int step,
+                      double fovy, const double* cam_pos, const double* cam_mat, double z_min, int W, int H, int R, int max_draws, int B, int* action,
+                      unsigned char* is_random, unsigned char* exhausted, void* stream);
 /* output.view(-1).max(0) per image (Grasping_Agent_multidiscrete.py:295-299): q [B,n] -> idx [B] int32 (rot*HW + y*W + x), val [B] f32 */
 int gq_argmax(const float* q, int B, int n, int* idx, float* val, void* stream);
 

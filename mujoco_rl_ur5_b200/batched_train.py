@@ -1,0 +1,263 @@
+"""BatchedTrainer: the reference's online training loop (Grasping_Agent_multidiscrete.main, :515-583) over N device environments.
+
+Per transition the reference runs  transform_observation -> epsilon_greedy -> env.step -> memory.push -> learn().  Here one batched step
+does that for N envs at once, every part a kernel of this project:
+    gq_obs_to_state_keyed (acting state = the state that is stored) -> QNetForward with per-image BatchNorm on the learner's current
+    weights, in chunks -> gq_argmax -> gq_sample_actions (epsilon-greedy, depth-filtered random actions) -> BatchedGraspEnv.step ->
+    ObservationReplay.push_batch -> `updates_per_step` x QNetLearner.learn_step on ObservationReplay.sample(batch_size).
+Every random choice (depth noise, ColorJitter, the epsilon draw, the random-action candidates) is keyed on (seed, global env index,
+step), so the actions and states of an env do not depend on how the envs are batched or sharded over GPUs.
+
+Transition numbers: env g (global index) of batched step t takes number n = steps_done + t * N_total + g, where steps_done is the count
+at the start or the resume; its epsilon is EPS_END + (EPS_START - EPS_END) exp(-n / EPS_DECAY) as in epsilon_greedy (:244-246), and
+its keyed step counter is the number of the batch's first transition.  Checkpoints are the reference's main() dict (:560-572).
+
+Cost: updates_per_step defaults to n_envs, the reference's one learn() per transition.  A learn() step of batch 12 is a forward and
+backward of the whole network, so at that ratio the learner dominates a batched step; DESIGN.md section 5 gives measured times.
+
+Multi-GPU (torchrun): rank r runs envs [r N, (r + 1) N) of N_total = world N, the learner all-reduces its gradients over the process
+group, each rank keeps its own replay and sampling stream random.Random(seed + rank), the counters are summed when a checkpoint is
+written and rank 0 writes it.
+"""
+import argparse
+import json
+import math
+import random
+import sys
+from collections import defaultdict
+
+import numpy as np
+
+from .batched_env import BatchedGraspEnv
+from .qnet_learn import QNetLearner
+from .replay_buffer import ObservationReplay
+
+EPS_START, EPS_END, EPS_DECAY = 1.0, 0.2, 8000   # Grasping_Agent_multidiscrete.py:35-37
+COUNTERS = ("greedy_rotations", "greedy_rotations_successes", "random_rotations_successes")
+
+
+def epsilon(n, eps_start=EPS_START, eps_end=EPS_END, eps_decay=EPS_DECAY):
+    """the reference's exploration rate of transition n (epsilon_greedy, :244-246), with its arithmetic (math.exp of -1.0 n / decay)"""
+    return eps_end + (eps_start - eps_end) * math.exp(-1.0 * n / eps_decay)
+
+
+def load_checkpoint(path_or_dict):
+    import torch
+
+    if isinstance(path_or_dict, dict):
+        return path_or_dict
+    return torch.load(path_or_dict, map_location="cpu", weights_only=False)
+
+
+class BatchedTrainer:
+    def __init__(self, n_envs, scene="A", device=0, seed=0, batch_size=12, mem_size=None, updates_per_step=None, lr=1e-3, eps_start=EPS_START,
+                 eps_end=EPS_END, eps_decay=EPS_DECAY, load=None, env_index_offset=None, n_total=None, process_group=None, chunk=64, max_draws=256,
+                 noise_std=0.001, log=None):
+        import torch
+        import torch.distributed as dist
+
+        self.torch = torch
+        self.pg = process_group
+        rank, world = (dist.get_rank(process_group), dist.get_world_size(process_group)) if process_group is not None else (0, 1)
+        self.rank = rank
+        self.n_envs = int(n_envs)
+        self.env_offset = rank * self.n_envs if env_index_offset is None else int(env_index_offset)
+        self.n_total = world * self.n_envs if n_total is None else int(n_total)
+        self.env = BatchedGraspEnv(self.n_envs, scene, device, env_index_offset=self.env_offset)
+        self.dev = self.env.engine.device
+        self.seed = int(seed)
+        self.batch_size = int(batch_size)
+        self.updates_per_step = self.n_envs if updates_per_step is None else int(updates_per_step)
+        self.eps_start, self.eps_end, self.eps_decay = eps_start, eps_end, eps_decay
+        self.chunk, self.max_draws, self.noise_std = int(chunk), int(max_draws), float(noise_std)
+        self.log = log
+        ckpt = None if load is None else load_checkpoint(load)
+        if ckpt is None:
+            self.learner = QNetLearner(None, device, lr=lr, seed=self.seed, process_group=process_group)
+        else:  # as the reference's constructor: the optimizer state (and with it the learning rate) comes from the checkpoint (:157-179)
+            self.learner = QNetLearner.from_checkpoint(ckpt, device, process_group=process_group)
+        ckpt = ckpt or {}
+        self.steps_done = int(ckpt.get("step", 0))
+        # as the reference (:161-163, :182): EPS_START for a fresh agent, the checkpoint's value or EPS_STEADY = 0 for a loaded one
+        self.eps_threshold = float(ckpt.get("epsilon", 0.0)) if ckpt else float(eps_start)
+        # counters restored from the checkpoint (the same on every rank) and counted in this run (summed over the ranks when saved)
+        self.base_counters = {k: defaultdict(int, {str(r): int(v) for r, v in (ckpt.get(k) or {}).items()}) for k in COUNTERS}
+        self.run_counts = np.zeros((len(COUNTERS), len(self.env.rotations)), dtype=np.int64)
+        mem = max(2000, 4 * self.n_envs) if mem_size is None else int(mem_size)
+        W, H = self.env.IMAGE_WIDTH, self.env.IMAGE_HEIGHT
+        self.replay = ObservationReplay(mem, (H, W), device=self.dev, rng=random.Random(self.seed + rank))
+        A = self.env.arrays
+        cam = self.env.cam
+        self.camera = (float(np.asarray(A["cam_fovy"]).ravel()[cam]), np.asarray(A["cam_pos0"], dtype=np.float64).reshape(-1, 3)[cam],
+                       np.asarray(A["cam_mat0"], dtype=np.float64).reshape(-1, 9)[cam])
+        self.z_min = self.env.TABLE_HEIGHT - 0.01                               # :275
+        self.depth_threshold = float(np.round(self.camera[1][2] - self.env.TABLE_HEIGHT + 0.01, 3))  # :130-135
+        self.genv = self.env_offset + torch.arange(self.n_envs, dtype=torch.int64, device=self.dev)
+        self.batched_steps = 0
+
+    # ------------------------------------------------------------------ acting
+    def acting_states(self, obs, step):
+        """the keyed training transform of the observation: what the agent acts on and what the replay regenerates"""
+        t = self.torch
+        return self.learner.fw.obs_to_state_keyed(obs["rgb"], obs["depth"], self.genv, t.full((self.n_envs,), step, dtype=t.int64, device=self.dev),
+                                                  self.seed, depth_threshold=self.depth_threshold, noise_std=self.noise_std)
+
+    def greedy_indices(self, states):
+        """flat arg-max rot*H*W + y*W + x per image, forward and arg-max chunk by chunk (the Q-maps of all envs are never held at once)"""
+        t = self.torch
+        fw = self.learner.fw
+        idx = t.empty(states.shape[0], dtype=t.int32, device=self.dev)
+        val = t.empty(states.shape[0], dtype=t.float32, device=self.dev)
+        for i in range(0, states.shape[0], self.chunk):
+            q = fw.forward(states[i:i + self.chunk])
+            fw._ck(fw.L.gq_argmax(fw._p(q), q.shape[0], q[0].numel(), fw._p(idx[i:]), fw._p(val[i:]), fw._stream()), "gq_argmax")
+        return idx
+
+    def epsilons(self):
+        """epsilon of every env's transition in the current batched step"""
+        base = self.steps_done + self.env_offset
+        return [epsilon(base + i, self.eps_start, self.eps_end, self.eps_decay) for i in range(self.n_envs)]
+
+    def act(self, obs):
+        """-> (acting states, actions [N,2] int32, is_random [N] bool, exhausted [N] bool) for the current batched step"""
+        t = self.torch
+        step = self.steps_done & 0xFFFFFFFF
+        states = self.acting_states(obs, step)
+        idx = self.greedy_indices(states)
+        eps = t.tensor(self.epsilons(), dtype=t.float64)
+        act, rnd, exh = self.learner.fw.sample_actions(obs["depth"], idx, eps, self.genv, step, self.seed, self.camera, self.z_min,
+                                                       len(self.env.rotations), self.max_draws)
+        return states, act, rnd, exh
+
+    # ------------------------------------------------------------------ one batched step
+    def step(self, mark=None):
+        """one batched step; `mark(name)` (optional) is called after each phase - "act", "env_step", "push", "learn" - and before the first
+        with "start" (tools/train_profile.py records a CUDA event there)"""
+        t = self.torch
+        mark = mark or (lambda name: None)
+        env = self.env
+        obs = env.current_observation
+        key = self.steps_done & 0xFFFFFFFF
+        mark("start")
+        _, act, rnd, exh = self.act(obs)
+        mark("act")
+        _, reward, _, _ = env.step(act)
+        mark("env_step")
+        HW = env.IMAGE_WIDTH * env.IMAGE_HEIGHT
+        flat = act[:, 1].to(t.int64) * HW + act[:, 0].to(t.int64)
+        self.replay.push_batch(obs["rgb"], obs["depth"], flat, t.from_numpy(reward.astype(np.float32)), self.genv,
+                               t.full((self.n_envs,), key, dtype=t.int64))
+        mark("push")
+        losses = []
+        if len(self.replay) >= 2 * self.batch_size:  # :396-399
+            for _ in range(self.updates_per_step):
+                s, a, r = self.replay.sample(self.batch_size, self.learner.fw, self.seed, self.depth_threshold, self.noise_std)
+                losses.append(self.learner.learn_step(s, a, r))
+        mark("learn")
+        # update_tensorboard's counters (:448-466), keyed by str(rotation) like the reference's defaultdicts
+        rot = act[:, 1].cpu().numpy()
+        rnd_h, exh_h = rnd.cpu().numpy(), exh.cpu().numpy()
+        ok = reward == 1
+        R = len(env.rotations)
+        self.run_counts[0] += np.bincount(rot[~rnd_h], minlength=R)[:R]
+        self.run_counts[1] += np.bincount(rot[~rnd_h & ok], minlength=R)[:R]
+        self.run_counts[2] += np.bincount(rot[rnd_h & ok], minlength=R)[:R]
+        self.steps_done += self.n_total
+        self.eps_threshold = epsilon(self.steps_done - 1, self.eps_start, self.eps_end, self.eps_decay)  # the last transition's, as the reference keeps it
+        self.batched_steps += 1
+        self.last_step = {"actions": act.cpu().numpy(), "is_random": rnd_h, "exhausted": exh_h, "reward": reward}
+        mean = lambda m: float(reward[m].mean()) if m.any() else None
+        rec = {"rank": self.rank, "step": self.batched_steps, "steps_done": self.steps_done, "epsilon": self.eps_threshold, "n_greedy": int((~rnd_h).sum()),
+               "n_random": int(rnd_h.sum()), "n_exhausted": int(exh_h.sum()), "mean_reward_greedy": mean(~rnd_h), "mean_reward_random": mean(rnd_h),
+               "updates": len(losses), "mean_loss": float(np.mean(losses)) if losses else None}
+        if self.log is not None:
+            self.log.write(json.dumps(rec) + "\n")
+            self.log.flush()
+        return rec
+
+    def train(self, episodes, steps_per_episode):
+        for _ in range(episodes):
+            self.env.reset()
+            for _ in range(steps_per_episode):
+                self.step()
+
+    # ------------------------------------------------------------------ checkpoints
+    def counters(self):
+        """the three rotation counters (dicts str(rot) -> count) of the reference, this run's counts summed over the ranks"""
+        t = self.torch
+        counts = self.run_counts
+        if self.pg is not None:
+            import torch.distributed as dist
+
+            c = t.from_numpy(counts).to(self.dev)
+            dist.all_reduce(c, op=dist.ReduceOp.SUM, group=self.pg)
+            counts = c.cpu().numpy()
+        out = {}
+        for i, k in enumerate(COUNTERS):
+            d = defaultdict(int, self.base_counters[k])
+            for r in range(counts.shape[1]):
+                if counts[i, r]:
+                    d[str(r)] += int(counts[i, r])
+            out[k] = d
+        return out
+
+    def checkpoint(self):
+        """the dict the reference's main() saves (:560-572)"""
+        ck = self.learner.checkpoint()
+        return {"step": self.steps_done, "model_state_dict": ck["model_state_dict"], "optimizer_state_dict": ck["optimizer_state_dict"],
+                "epsilon": self.eps_threshold, **self.counters()}
+
+    def save(self, path):
+        """writes the checkpoint from rank 0 (every rank must call it: the counters are summed over the ranks)"""
+        ck = self.checkpoint()
+        if self.rank == 0:
+            self.torch.save(ck, path)
+        return ck
+
+    def close(self):
+        self.env.close()
+
+
+def main(argv=None):
+    p = argparse.ArgumentParser(prog="python -m mujoco_rl_ur5_b200.batched_train", description=__doc__.split("\n")[0])
+    p.add_argument("--envs", type=int, default=256, help="environments per GPU")
+    p.add_argument("--scene", default="A")
+    p.add_argument("--episodes", type=int, default=1)
+    p.add_argument("--steps-per-episode", type=int, default=50)
+    p.add_argument("--updates-per-step", type=int, default=None, help="learn() calls per batched step (default: --envs, one per transition)")
+    p.add_argument("--batch-size", type=int, default=12)
+    p.add_argument("--mem-size", type=int, default=None, help="replay capacity per GPU (default: max(2000, 4 envs))")
+    p.add_argument("--lr", type=float, default=1e-3)
+    p.add_argument("--eps-start", type=float, default=EPS_START)
+    p.add_argument("--eps-end", type=float, default=EPS_END)
+    p.add_argument("--eps-decay", type=float, default=EPS_DECAY)
+    p.add_argument("--seed", type=int, default=0)
+    p.add_argument("--load", default=None, help="checkpoint to resume from (the reference's or this trainer's)")
+    p.add_argument("--out", default=None, help="checkpoint written at the end")
+    a = p.parse_args(argv)
+    import os
+
+    import torch
+    import torch.distributed as dist
+
+    pg, device = None, 0
+    if int(os.environ.get("WORLD_SIZE", "1")) > 1:  # torchrun
+        device = int(os.environ.get("LOCAL_RANK", "0"))
+        torch.cuda.set_device(device)
+        dist.init_process_group("nccl")
+        pg = dist.group.WORLD
+    tr = BatchedTrainer(a.envs, a.scene, device, seed=a.seed, batch_size=a.batch_size, mem_size=a.mem_size, updates_per_step=a.updates_per_step, lr=a.lr,
+                        eps_start=a.eps_start, eps_end=a.eps_end, eps_decay=a.eps_decay, load=a.load, process_group=pg,
+                        log=sys.stdout if (pg is None or dist.get_rank() == 0) else None)
+    try:
+        tr.train(a.episodes, a.steps_per_episode)
+        if a.out:
+            tr.save(a.out)
+    finally:
+        tr.close()
+        if pg is not None:
+            dist.destroy_process_group()
+
+
+if __name__ == "__main__":
+    main()

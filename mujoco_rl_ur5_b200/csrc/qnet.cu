@@ -565,25 +565,78 @@ __device__ __forceinline__ void jitter_op(int op, float f, float mean, float& r,
     b = i == 0 ? pp : i == 1 ? pp : i == 2 ? t : i == 3 ? v : i == 4 ? v : q;
   }
 }
-// per image: min / max of the noisy negated clipped depth, and the grey mean of the image as it is when the contrast operation runs
+// ---- keyed draws: every random decision of the online trainer is a function of (seed, global env, step), like the depth noise.
+// Counter (c0, env_lo, env_hi, step), key (seed_lo, seed_hi) of philox4x32_10.  The depth noise uses c0 = pixel < 2^31; the draws below
+// use c0 = 0x80000000 + j, so the two streams never overlap:
+//   j = 0      w0 -> epsilon uniform u (the transition is greedy iff u > eps); w1, w2, w3 -> brightness, contrast, saturation factors
+//   j = 1      w0 -> hue factor; w1 -> operation order = permutation number (uint64)w1 * 24 >> 32 of (0,1,2,3), permutations in
+//              lexicographic order (0 = 0123, 1 = 0132, ..., 23 = 3210)
+//   j = 2 + k  w0 -> k-th random-action candidate (uint64)w0 * (W*H*R) >> 32 (flat action rot*W*H + y*W + x)
+// Uniforms are ((w >> 8) + 0.5) / 2^24 in float, as in obs_noise; factors 0.5 + u (brightness, contrast, saturation: 1 +- 0.5) and
+// u - 0.5 (hue: +-0.5), the ranges of ColorJitter(0.5, 0.5, 0.5, 0.5).  tests/test_batched_train.py restates this table in numpy.
+#define KEYED_C0 0x80000000u
+__device__ __forceinline__ void keyed_words(uint64_t seed, uint64_t env, uint32_t step, uint32_t j, uint32_t* w) {
+  philox4x32_10(KEYED_C0 + j, (uint32_t)env, (uint32_t)(env >> 32), step, (uint32_t)seed, (uint32_t)(seed >> 32), w);
+}
+__device__ __forceinline__ float keyed_uniform(uint32_t w) { return ((float)(w >> 8) + 0.5f) * (1.0f / 16777216.0f); }
+// the ColorJitter factors (brightness, contrast, saturation, hue) and operation order of one (env, step)
+__device__ void keyed_jitter(uint64_t seed, uint64_t env, uint32_t step, float* fac, int* ord) {
+  uint32_t w[4], v[4];
+  keyed_words(seed, env, step, 0, w);
+  keyed_words(seed, env, step, 1, v);
+  fac[0] = 0.5f + keyed_uniform(w[1]); fac[1] = 0.5f + keyed_uniform(w[2]); fac[2] = 0.5f + keyed_uniform(w[3]);
+  fac[3] = keyed_uniform(v[0]) - 0.5f;
+  int p = (int)(((uint64_t)v[1] * 24u) >> 32), left = 0x3210;  // factorial-base digits 6, 2, 1 pick from the unused operations (nibbles)
+  const int radix[3] = {6, 2, 1};
+#pragma unroll
+  for (int k = 0; k < 3; k++) {
+    const int d = p / radix[k];
+    p -= d * radix[k];
+    ord[k] = (left >> (4 * d)) & 15;
+    const int lowmask = (1 << (4 * d)) - 1;
+    left = (left & lowmask) | ((left >> 4) & ~lowmask);  // drop nibble d
+  }
+  ord[3] = left & 15;
+}
+
+// per image: min / max of the noisy negated clipped depth, and the grey mean of the image as it is when the contrast operation runs.
+// Row b reads image slot[b] (NULL: b) and is keyed on env_index[b] (NULL: b) and steps[b] (NULL: step).  With draw_fac / draw_ord
+// the row's factors and order are the keyed draws of (seed, env, step), written there for k_obs_train_state; otherwise they come
+// from jitter / order.
 __global__ void __launch_bounds__(256) k_obs_train_reduce(const unsigned char* __restrict__ rgb, const float* __restrict__ depth, int HW, float thr, float noise_std,
-                                                          unsigned long long seed, const long long* __restrict__ env_index, unsigned int step,
-                                                          const float* __restrict__ jitter, const int* __restrict__ order, float* __restrict__ red) {
+                                                          unsigned long long seed, const long long* __restrict__ slot, const long long* __restrict__ env_index,
+                                                          const unsigned int* __restrict__ steps, unsigned int step, const float* __restrict__ jitter,
+                                                          const int* __restrict__ order, float* __restrict__ draw_fac, int* __restrict__ draw_ord,
+                                                          float* __restrict__ red) {
   __shared__ float smin[256], smax[256];
   __shared__ double ssum[256];
+  __shared__ float sfac[4];
+  __shared__ int sord[4];
   const int b = blockIdx.x;
+  const size_t s = slot ? (size_t)slot[b] : (size_t)b;
   const unsigned long long env = env_index ? (unsigned long long)env_index[b] : (unsigned long long)b;
+  if (steps) step = steps[b];
   int ord[4] = {0, 1, 2, 3};
   float fac[4] = {1.f, 1.f, 1.f, 0.f};
-  if (jitter) for (int k = 0; k < 4; k++) fac[k] = jitter[4 * b + k];
-  if (order) for (int k = 0; k < 4; k++) ord[k] = order[4 * b + k];
+  if (draw_fac) {
+    if (threadIdx.x == 0) {
+      keyed_jitter(seed, env, step, sfac, sord);
+      for (int k = 0; k < 4; k++) { draw_fac[4 * b + k] = sfac[k]; draw_ord[4 * b + k] = sord[k]; }
+    }
+    __syncthreads();
+    for (int k = 0; k < 4; k++) { fac[k] = sfac[k]; ord[k] = sord[k]; }
+  } else {
+    if (jitter) for (int k = 0; k < 4; k++) fac[k] = jitter[4 * b + k];
+    if (order) for (int k = 0; k < 4; k++) ord[k] = order[4 * b + k];
+  }
+  const bool jit = draw_fac || jitter;  // ColorJitter applied (drawn here or given)
   float lo = 3.0e38f, hi = -3.0e38f;
   double gs = 0;
   for (int i = threadIdx.x; i < HW; i += blockDim.x) {
-    float v = -(fminf(depth[(size_t)b * HW + i], thr) + noise_std * obs_noise(seed, env, step, (uint32_t)i));
+    float v = -(fminf(depth[s * HW + i], thr) + noise_std * obs_noise(seed, env, step, (uint32_t)i));
     lo = fminf(lo, v); hi = fmaxf(hi, v);
-    if (jitter) {
-      const unsigned char* px = rgb + ((size_t)b * HW + i) * 3;
+    if (jit) {
+      const unsigned char* px = rgb + (s * HW + i) * 3;
       float r = px[0] * (1.f / 255.f), g = px[1] * (1.f / 255.f), bl = px[2] * (1.f / 255.f);
       for (int k = 0; k < 4 && ord[k] != 1; k++) jitter_op(ord[k], fac[ord[k]], 0.f, r, g, bl);  // the operations in front of contrast
       gs += gray_of(r, g, bl);
@@ -601,19 +654,22 @@ __global__ void __launch_bounds__(256) k_obs_train_reduce(const unsigned char* _
   if (threadIdx.x == 0) { red[4 * b] = smin[0]; red[4 * b + 1] = smax[0]; red[4 * b + 2] = (float)(ssum[0] / HW); red[4 * b + 3] = 0.f; }
 }
 __global__ void k_obs_train_state(const unsigned char* __restrict__ rgb, const float* __restrict__ depth, const float* __restrict__ red, float thr, float noise_std,
-                                  unsigned long long seed, const long long* __restrict__ env_index, unsigned int step, const float* __restrict__ jitter,
-                                  const int* __restrict__ order, int B, int HW, float* __restrict__ state, bf16* __restrict__ state_nhwc) {
+                                  unsigned long long seed, const long long* __restrict__ slot, const long long* __restrict__ env_index,
+                                  const unsigned int* __restrict__ steps, unsigned int step, const float* __restrict__ jitter, const int* __restrict__ order, int B,
+                                  int HW, float* __restrict__ state, bf16* __restrict__ state_nhwc) {
   size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= (size_t)B * HW) return;
   const int b = i / HW, p = i % HW;
+  const size_t src = (slot ? (size_t)slot[b] : (size_t)b) * HW + p;
   const unsigned long long env = env_index ? (unsigned long long)env_index[b] : (unsigned long long)b;
-  float r = rgb[3 * i] * (1.f / 255.f), g = rgb[3 * i + 1] * (1.f / 255.f), bl = rgb[3 * i + 2] * (1.f / 255.f);
+  if (steps) step = steps[b];
+  float r = rgb[3 * src] * (1.f / 255.f), g = rgb[3 * src + 1] * (1.f / 255.f), bl = rgb[3 * src + 2] * (1.f / 255.f);
   if (jitter) {
     const float mean = red[4 * b + 2];
     for (int k = 0; k < 4; k++) { const int op = order ? order[4 * b + k] : k; jitter_op(op, jitter[4 * b + op], mean, r, g, bl); }
   }
   const float lo = red[4 * b], hi = red[4 * b + 1];
-  const float d = (-(fminf(depth[i], thr) + noise_std * obs_noise(seed, env, step, (uint32_t)p)) - lo) / (hi - lo);
+  const float d = (-(fminf(depth[src], thr) + noise_std * obs_noise(seed, env, step, (uint32_t)p)) - lo) / (hi - lo);
   if (state) {
     float* out = state + (size_t)b * 4 * HW + p;
     out[0] = r; out[HW] = g; out[2 * (size_t)HW] = bl; out[3 * (size_t)HW] = d;
@@ -624,15 +680,96 @@ __global__ void k_obs_train_state(const unsigned char* __restrict__ rgb, const f
   }
 }
 
+// ---- Grasp_Agent.epsilon_greedy (Grasping_Agent_multidiscrete.py:232-282) for a batch, one warp per env.  Greedy iff the keyed
+// uniform u > eps[b]; otherwise the reference's rejection sampling: candidate k (keyed draw j = 2 + k) is accepted when its pixel's
+// world z >= z_min.  The 32 lanes test candidates 32 at a time and the lowest accepted k wins, which is the first accepted candidate
+// of the sequential loop.  After max_draws rejections the last candidate is taken and `exhausted` set.
+struct SampleCam { double fovy, pos[3], mat[9]; };
+// z of pixel_2_world with the arithmetic of the engine's k_pixel_2_world (grasp_engine.cu): the same expressions, so that the accept
+// decisions equal ge_pixel_2_world's
+__device__ __forceinline__ double pixel_world_z(const SampleCam& c, int W, int H, int px, int py, float depth) {
+  const double PI = 3.14159265358979323846;
+  double f = 0.5 * H / tan(c.fovy * PI / 360.0), d = -(double)depth;
+  double pc[3] = {(px * d - 0.5 * W * d) / f, (py * d - 0.5 * H * d) / f, d}, t[3];
+  t[0] = pc[0] + c.pos[0]; t[1] = pc[1] + c.pos[1]; t[2] = pc[2] + c.pos[2];
+  return c.mat[2] * t[0] + c.mat[5] * t[1] + c.mat[8] * t[2];
+}
+__global__ void __launch_bounds__(256) k_sample_actions(const float* __restrict__ depth, const int* __restrict__ greedy_idx, const double* __restrict__ eps,
+                                                        unsigned long long seed, const long long* __restrict__ env_index, unsigned int step, SampleCam cam,
+                                                        double z_min, int W, int H, int R, int max_draws, int B, int* __restrict__ action,
+                                                        unsigned char* __restrict__ is_random, unsigned char* __restrict__ exhausted) {
+  const int b = (int)((blockIdx.x * (size_t)blockDim.x + threadIdx.x) >> 5), lane = threadIdx.x & 31;
+  if (b >= B) return;
+  const int HW = W * H;
+  const unsigned long long env = env_index ? (unsigned long long)env_index[b] : (unsigned long long)b;
+  uint32_t w[4];
+  keyed_words(seed, env, step, 0, w);
+  int flat;
+  bool rnd = !(keyed_uniform(w[0]) > eps[b]), none = false;
+  if (!rnd) {
+    flat = greedy_idx[b];
+  } else {
+    const float* dimg = depth + (size_t)b * HW;
+    const uint32_t n_act = (uint32_t)(HW * R);
+    flat = -1;
+    for (int base = 0; base < max_draws; base += 32) {
+      const int k = base + lane;
+      keyed_words(seed, env, step, 2u + (uint32_t)k, w);
+      const int cand = (int)(((uint64_t)w[0] * n_act) >> 32), a1 = cand % HW, x = a1 % W, y = a1 / W;
+      const bool ok = k < max_draws && pixel_world_z(cam, W, H, x, y, __ldg(dimg + a1)) >= z_min;
+      const unsigned acc = __ballot_sync(0xffffffffu, ok);
+      if (acc) { flat = __shfl_sync(0xffffffffu, cand, __ffs(acc) - 1); break; }
+      if (base + 32 >= max_draws) { flat = __shfl_sync(0xffffffffu, cand, (max_draws - 1) - base); none = true; }
+    }
+  }
+  if (lane == 0) {
+    action[2 * b] = flat % HW; action[2 * b + 1] = flat / HW;
+    is_random[b] = rnd; exhausted[b] = none;
+  }
+}
+
 // ------------------------------------------------------------------------------------------------ C-ABI
 extern "C" int gq_obs_to_state_train(const unsigned char* rgb, const float* depth, float depth_threshold, float noise_std, unsigned long long seed,
                                      const long long* env_index, unsigned int step, const float* jitter, const int* order, float* scratch_red,
                                      float* state, void* state_nhwc_bf16, int B, int HW, void* stream) {
   if (!rgb || !depth || !scratch_red || (!state && !state_nhwc_bf16) || B <= 0 || HW <= 0) { snprintf(q_err, sizeof q_err, "gq_obs_to_state_train: bad argument"); return -1; }
   cudaStream_t st = (cudaStream_t)stream;
-  k_obs_train_reduce<<<B, 256, 0, st>>>(rgb, depth, HW, depth_threshold, noise_std, seed, env_index, step, jitter, order, scratch_red);
-  k_obs_train_state<<<(unsigned)(((size_t)B * HW + 255) / 256), 256, 0, st>>>(rgb, depth, scratch_red, depth_threshold, noise_std, seed, env_index, step, jitter, order,
-                                                                              B, HW, state, (bf16*)state_nhwc_bf16);
+  k_obs_train_reduce<<<B, 256, 0, st>>>(rgb, depth, HW, depth_threshold, noise_std, seed, nullptr, env_index, nullptr, step, jitter, order, nullptr, nullptr,
+                                        scratch_red);
+  k_obs_train_state<<<(unsigned)(((size_t)B * HW + 255) / 256), 256, 0, st>>>(rgb, depth, scratch_red, depth_threshold, noise_std, seed, nullptr, env_index, nullptr,
+                                                                              step, jitter, order, B, HW, state, (bf16*)state_nhwc_bf16);
+  QCK(cudaGetLastError());
+  return 0;
+}
+extern "C" int gq_obs_to_state_keyed(const unsigned char* rgb, const float* depth, const long long* slot, const long long* env_index, const unsigned int* step,
+                                     float depth_threshold, float noise_std, unsigned long long seed, float* scratch_red, float* jitter_out, int* order_out,
+                                     float* state, void* state_nhwc_bf16, int B, int HW, void* stream) {
+  if (!rgb || !depth || !env_index || !step || !scratch_red || !jitter_out || !order_out || (!state && !state_nhwc_bf16) || B <= 0 || HW <= 0) {
+    snprintf(q_err, sizeof q_err, "gq_obs_to_state_keyed: bad argument");
+    return -1;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  k_obs_train_reduce<<<B, 256, 0, st>>>(rgb, depth, HW, depth_threshold, noise_std, seed, slot, env_index, step, 0u, nullptr, nullptr, jitter_out, order_out,
+                                        scratch_red);
+  k_obs_train_state<<<(unsigned)(((size_t)B * HW + 255) / 256), 256, 0, st>>>(rgb, depth, scratch_red, depth_threshold, noise_std, seed, slot, env_index, step,
+                                                                              0u, jitter_out, order_out, B, HW, state, (bf16*)state_nhwc_bf16);
+  QCK(cudaGetLastError());
+  return 0;
+}
+extern "C" int gq_sample_actions(const float* depth, const int* greedy_idx, const double* eps, unsigned long long seed, const long long* env_index,
+                                 unsigned int step, double fovy, const double* cam_pos, const double* cam_mat, double z_min, int W, int H, int R, int max_draws,
+                                 int B, int* action, unsigned char* is_random, unsigned char* exhausted, void* stream) {
+  if (!depth || !greedy_idx || !eps || !env_index || !cam_pos || !cam_mat || !action || !is_random || !exhausted || W <= 0 || H <= 0 || R <= 0 ||
+      max_draws <= 0 || B <= 0 || (long long)W * H * R > 0x7fffffffLL) {
+    snprintf(q_err, sizeof q_err, "gq_sample_actions: bad argument");
+    return -1;
+  }
+  SampleCam cam;
+  cam.fovy = fovy;
+  for (int k = 0; k < 3; k++) cam.pos[k] = cam_pos[k];
+  for (int k = 0; k < 9; k++) cam.mat[k] = cam_mat[k];
+  k_sample_actions<<<(unsigned)(((size_t)B * 32 + 255) / 256), 256, 0, (cudaStream_t)stream>>>(depth, greedy_idx, eps, seed, env_index, step, cam, z_min, W, H, R,
+                                                                                                max_draws, B, action, is_random, exhausted);
   QCK(cudaGetLastError());
   return 0;
 }

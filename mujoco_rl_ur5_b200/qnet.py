@@ -23,7 +23,8 @@ import numpy as np
 _HERE = os.path.dirname(os.path.abspath(__file__))
 QLIB_PATH = os.path.join(_HERE, "csrc", "libgrasp_qnet.so")
 _QLIB = None
-QSYMBOLS = ["gq_last_error", "gq_version", "gq_conv_partials_floats", "gq_conv_tc", "gq_conv_tc_block_out", "gq_conv_first", "gq_maxpool", "gq_bn_act", "gq_upsample2x", "gq_head", "gq_head_up2", "gq_argmax", "gq_obs_to_state", "gq_obs_to_state_train", "gq_conv_tc_fused"]
+QSYMBOLS = ["gq_last_error", "gq_version", "gq_conv_partials_floats", "gq_conv_tc", "gq_conv_tc_block_out", "gq_conv_first", "gq_maxpool", "gq_bn_act", "gq_upsample2x", "gq_head", "gq_head_up2", "gq_argmax", "gq_obs_to_state", "gq_obs_to_state_train", "gq_conv_tc_fused",
+            "gq_obs_to_state_keyed", "gq_sample_actions"]
 
 
 def load_qnet_library():
@@ -49,6 +50,9 @@ def load_qnet_library():
         L.gq_argmax.argtypes = [P, I, I, P, P, P]
         L.gq_obs_to_state.argtypes = [P, P, F, P, P, I, I, P]
         L.gq_obs_to_state_train.argtypes = [P, P, F, F, C.c_uint64, P, C.c_uint32, P, P, P, P, P, I, I, P]
+        L.gq_obs_to_state_keyed.argtypes = [P, P, P, P, P, F, F, C.c_uint64, P, P, P, P, P, I, I, P]
+        D = C.c_double
+        L.gq_sample_actions.argtypes = [P, P, P, C.c_uint64, P, C.c_uint32, D, P, P, D, I, I, I, I, I, P, P, P, P]
         _QLIB = L
     return _QLIB
 
@@ -347,6 +351,47 @@ class QNetForward:
                                               self._stream()), "gq_obs_to_state_train")
         self.launches += 1
         return (state, nhwc) if nhwc_bf16 else state
+
+    def obs_to_state_keyed(self, rgb, depth, env_index, step, seed, slot=None, depth_threshold=1.1, noise_std=0.001, return_draws=False):
+        """the training transform with the ColorJitter factors and order drawn from the keyed generator (gq_obs_to_state_keyed): row b is
+        image slot[b] of rgb [S,H,W,3] u8 / depth [S,H,W] f32 (slot None: b), keyed on env_index[b] and step[b] (int64 / uint32 tensors
+        or sequences of B).  -> state [B,4,H,W] f32, and (factors [B,4] f32, order [B,4] int32) with return_draws=True"""
+        t = self.torch
+        rgb, depth = rgb.contiguous(), depth.contiguous()
+        H, W = depth.shape[1], depth.shape[2]
+        ei = t.as_tensor(env_index).to(self.dev, t.int64).contiguous()
+        B = ei.numel()
+        st = t.as_tensor(step).to(self.dev, t.int64).reshape(B).bitwise_and(0xFFFFFFFF).to(t.int32).contiguous()  # the uint32 bit pattern
+        sl = None if slot is None else t.as_tensor(slot).to(self.dev, t.int64).contiguous()
+        state = t.empty((B, 4, H, W), dtype=t.float32, device=self.dev)
+        red = t.empty((B, 4), dtype=t.float32, device=self.dev)
+        fac = t.empty((B, 4), dtype=t.float32, device=self.dev)
+        order = t.empty((B, 4), dtype=t.int32, device=self.dev)
+        self._ck(self.L.gq_obs_to_state_keyed(self._p(rgb), self._p(depth), self._p(sl), self._p(ei), self._p(st), float(depth_threshold), float(noise_std),
+                                              int(seed) & (2 ** 64 - 1), self._p(red), self._p(fac), self._p(order), self._p(state), None, B, H * W,
+                                              self._stream()), "gq_obs_to_state_keyed")
+        return (state, fac, order) if return_draws else state
+
+    def sample_actions(self, depth, greedy_idx, eps, env_index, step, seed, camera, z_min, n_rot=6, max_draws=256):
+        """epsilon-greedy selection (gq_sample_actions): depth [B,H,W] f32 of the current observation, greedy_idx [B] int32 (flat arg-max),
+        eps [B] f64, env_index [B] int64 global env ids, step / seed: the keyed generator's counter and key, camera = (fovy, pos[3],
+        mat[9]) of the top-down camera, z_min = TABLE_HEIGHT - 0.01.  -> (action [B,2] int32, is_random [B] bool, exhausted [B] bool)"""
+        t = self.torch
+        B, H, W = depth.shape
+        depth = depth.contiguous()
+        gi = greedy_idx.to(self.dev, t.int32).contiguous()
+        ep = t.as_tensor(eps, dtype=t.float64).to(self.dev).reshape(B).contiguous()
+        ei = t.as_tensor(env_index).to(self.dev, t.int64).reshape(B).contiguous()
+        fovy, pos, mat = camera
+        pos = (C.c_double * 3)(*[float(v) for v in np.asarray(pos).ravel()])
+        mat = (C.c_double * 9)(*[float(v) for v in np.asarray(mat).ravel()])
+        action = t.empty((B, 2), dtype=t.int32, device=self.dev)
+        rnd = t.empty(B, dtype=t.uint8, device=self.dev)
+        exh = t.empty(B, dtype=t.uint8, device=self.dev)
+        self._ck(self.L.gq_sample_actions(self._p(depth), self._p(gi), self._p(ep), int(seed) & (2 ** 64 - 1), self._p(ei), int(step) & 0xFFFFFFFF, float(fovy),
+                                          C.cast(pos, C.c_void_p), C.cast(mat, C.c_void_p), float(z_min), W, H, int(n_rot), int(max_draws), B, self._p(action),
+                                          self._p(rnd), self._p(exh), self._stream()), "gq_sample_actions")
+        return action, rnd.bool(), exh.bool()
 
     def greedy(self, q):
         """flat arg-max per image and its split into (pixel index, rotation index) as transform_action does

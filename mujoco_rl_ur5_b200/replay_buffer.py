@@ -11,21 +11,21 @@ environment pushes N transitions at once, and `sample` draws the SAME indices th
 positions through `randbelow` only, so sampling `range(len)` with the same generator state returns the indices of the
 elements the reference's list sampling returns.  By default the generator is Python's global `random` module seeded with
 20 exactly like the reference (the unchanged agent draws its epsilon from the same stream); pass `rng=random.Random(20)` for
-a private stream (a generator passed in is used as it is, never re-seeded).  Storage and gathers are tensor plumbing (any torch device); there is no kernel here.
+a private stream (a generator passed in is used as it is, never re-seeded).  DeviceReplayBuffer's storage and gathers are tensor plumbing
+(any torch device); ObservationReplay, the online trainer's memory, stores observations and regenerates states with a kernel.
 """
 import random as _random
 
 
-class DeviceReplayBuffer:
-    def __init__(self, size, state_shape=(4, 200, 200), device="cuda", state_dtype=None, rng=None, seed=20):
+class _Ring:
+    """the ring bookkeeping and the reference's sampling, shared by the buffers below (they differ in what a slot stores)"""
+
+    def __init__(self, size, device, rng, seed):
         import torch
 
         self.torch = torch
         self.size = int(size)
         self.device = torch.device(device)
-        self.states = torch.zeros((self.size,) + tuple(state_shape), dtype=state_dtype or torch.float32, device=self.device)
-        self.actions = torch.zeros(self.size, dtype=torch.int64, device=self.device)
-        self.rewards = torch.zeros(self.size, dtype=torch.float32, device=self.device)
         self.position = 0
         self.length = 0
         # Modules.py:33 seeds the GLOBAL stream with 20; a caller-supplied generator keeps its own state, seed=None skips seeding
@@ -35,6 +35,33 @@ class DeviceReplayBuffer:
 
     def __len__(self):
         return self.length
+
+    def _claim(self, n):
+        """slots of a push of n transitions in env order -> (skip, idx): the first `skip` transitions are overwritten within the same
+        push (n > size) and are not stored; the others go to the slots idx.  Advances the ring."""
+        t = self.torch
+        skip = max(0, n - self.size)
+        if skip:  # only the last `size` survive; the write position still advances by n
+            self.position = (self.position + skip) % self.size
+            n = self.size
+        idx = (self.position + t.arange(n, device=self.device)) % self.size
+        self.length = min(self.size, self.length + n)
+        self.position = (self.position + n) % self.size
+        return skip, idx
+
+    def sample_indices(self, batch_size):
+        idx = self.rng.sample(range(self.length), batch_size - 1)
+        idx.append((self.position - 1) % self.length)  # memory[position - 1]: the newest (Python's -1 when position == 0)
+        return idx
+
+
+class DeviceReplayBuffer(_Ring):
+    def __init__(self, size, state_shape=(4, 200, 200), device="cuda", state_dtype=None, rng=None, seed=20):
+        super().__init__(size, device, rng, seed)
+        torch = self.torch
+        self.states = torch.zeros((self.size,) + tuple(state_shape), dtype=state_dtype or torch.float32, device=self.device)
+        self.actions = torch.zeros(self.size, dtype=torch.int64, device=self.device)
+        self.rewards = torch.zeros(self.size, dtype=torch.float32, device=self.device)
 
     def push(self, state, action, reward):
         """one transition: state [4,H,W] or [1,4,H,W] (the agent's tensor), action / reward scalars or 1-element tensors"""
@@ -49,22 +76,10 @@ class DeviceReplayBuffer:
         states = states.to(self.device, self.states.dtype)
         actions = t.as_tensor(actions).to(self.device, t.int64).reshape(n)
         rewards = t.as_tensor(rewards).to(self.device, t.float32).reshape(n)
-        if n > self.size:  # only the last `size` survive; the write position still advances by n
-            skip = n - self.size
-            states, actions, rewards = states[skip:], actions[skip:], rewards[skip:]
-            self.position = (self.position + skip) % self.size
-            n = self.size
-        idx = (self.position + t.arange(n, device=self.device)) % self.size
-        self.states.index_copy_(0, idx, states)
-        self.actions.index_copy_(0, idx, actions)
-        self.rewards.index_copy_(0, idx, rewards)
-        self.length = min(self.size, self.length + n)
-        self.position = (self.position + n) % self.size
-
-    def sample_indices(self, batch_size):
-        idx = self.rng.sample(range(self.length), batch_size - 1)
-        idx.append((self.position - 1) % self.length)  # memory[position - 1]: the newest (Python's -1 when position == 0)
-        return idx
+        skip, idx = self._claim(n)
+        self.states.index_copy_(0, idx, states[skip:])
+        self.actions.index_copy_(0, idx, actions[skip:])
+        self.rewards.index_copy_(0, idx, rewards[skip:])
 
     def sample(self, batch_size):
         """-> (states [B,4,H,W], actions [B,1] int64, rewards [B,1] f32), in the reference's order (random ones, then the newest)"""
@@ -74,3 +89,45 @@ class DeviceReplayBuffer:
 
     def get(self, index):
         return self.states[index], self.actions[index], self.rewards[index]
+
+
+class ObservationReplay(_Ring):
+    """Replay memory of the online trainer: it stores the raw observation (rgb u8 [H,W,3], depth f32 [H,W]), the flat action, the
+    reward and the (global env, step) key of each transition - 280 024 B at 200x200 (rgb 120 000, depth 160 000, action int64, reward f32,
+    env int64, step int32 holding the uint32 key) against 640 012 B for the f32 state - and
+    regenerates the training state at sample time with gq_obs_to_state_keyed.  That transform is a function of the observation and
+    its key only, so a sampled state equals, bit for bit, the state the agent acted on when it pushed the transition.  Ring and
+    sampling are DeviceReplayBuffer's (the reference's B - 1 uniform picks plus the newest, from `rng`)."""
+
+    def __init__(self, size, image_hw=(200, 200), device="cuda", rng=None, seed=20):
+        super().__init__(size, device, rng, seed)
+        t = self.torch
+        H, W = image_hw
+        self.rgb = t.zeros((self.size, H, W, 3), dtype=t.uint8, device=self.device)
+        self.depth = t.zeros((self.size, H, W), dtype=t.float32, device=self.device)
+        self.actions = t.zeros(self.size, dtype=t.int64, device=self.device)
+        self.rewards = t.zeros(self.size, dtype=t.float32, device=self.device)
+        self.envs = t.zeros(self.size, dtype=t.int64, device=self.device)
+        self.steps = t.zeros(self.size, dtype=t.int32, device=self.device)  # the uint32 step key, bit for bit
+
+    def push_batch(self, rgb, depth, actions, rewards, envs, steps):
+        """N transitions in env order: observations [N,H,W,3] / [N,H,W], flat actions, rewards, global env ids and the step key"""
+        t = self.torch
+        n = int(depth.shape[0])
+        skip, idx = self._claim(n)
+        as_dev = lambda x, dt: t.as_tensor(x).to(self.device, dt).reshape(n)[skip:]
+        self.rgb.index_copy_(0, idx, rgb[skip:].to(self.device))
+        self.depth.index_copy_(0, idx, depth[skip:].to(self.device, t.float32))
+        self.actions.index_copy_(0, idx, as_dev(actions, t.int64))
+        self.rewards.index_copy_(0, idx, as_dev(rewards, t.float32))
+        self.envs.index_copy_(0, idx, as_dev(envs, t.int64))
+        self.steps.index_copy_(0, idx, as_dev(t.as_tensor(steps).to(t.int64).bitwise_and(0xFFFFFFFF).to(t.int32), t.int32))
+
+    def sample(self, batch_size, fwd, seed, depth_threshold=1.1, noise_std=0.001):
+        """-> (states [B,4,H,W] f32, actions [B,1] int64, rewards [B,1] f32) in the reference's order; the states are regenerated by
+        `fwd` (a QNetForward on this buffer's device) with the keyed transform under `seed`"""
+        t = self.torch
+        idx = t.as_tensor(self.sample_indices(batch_size), dtype=t.int64, device=self.device)
+        states = fwd.obs_to_state_keyed(self.rgb, self.depth, self.envs.index_select(0, idx), self.steps.index_select(0, idx), seed, slot=idx,
+                                        depth_threshold=depth_threshold, noise_std=noise_std)
+        return states, self.actions.index_select(0, idx)[:, None], self.rewards.index_select(0, idx)[:, None]

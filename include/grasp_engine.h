@@ -45,9 +45,12 @@ int ge_destroy(ge_handle h);
 /* model sizes: what = 0 nq, 1 nv, 2 nbody, 3 ngeom, 4 nu, 5 n_envs, 6 max contacts per env, 7 shared-memory bytes per env,
  * 8 environments (warps) per CTA of the sub-step kernel, 9 workspace placement (0 shared memory, 1 HBM rows: scenes whose per-env
  * workspace exceeds 227 KB, e.g. the 40-object scene), 10 hcap = doubles of the Newton Hessian block region in the workspace, 11 hfull =
- * nv (nv + 1) / 2 = doubles of one env's Hessian overflow row in HBM (CTA-per-env build: a Hessian build whose blocks add up to more
- * than hcap goes there).  The CTA-per-env build reads two overrides at ge_create: GE_MAXCON (contact capacity, 16..512) and GE_HCAP
- * (hcap, from Σ tree blocks + 6 maxcon + 64 up to hfull); a value outside its range is ignored, so size 6 / 10 tell what was used. */
+ * nv (nv + 1) / 2 = doubles of one env's Hessian overflow row in HBM (a Hessian build whose blocks add up to more than hcap goes
+ * there), 12 environments of the sub-step kernel resident per SM as granted by the occupancy API, 13 Hessian builds that used the
+ * overflow row since ge_create (synchronises the engine's stream; saturates at INT_MAX).  Both builds read GE_HCAP at ge_create (hcap,
+ * CTA-per-env build: from Σ tree blocks + 6 maxcon + 64 up to hfull; warp-per-env build: from the larger of Σ tree blocks and
+ * 6 maxcon + 6 nbody up to hfull); the CTA-per-env build also reads GE_MAXCON (contact capacity, 16..512).  A value outside its range
+ * is ignored, so size 6 / 10 tell what was used. */
 int ge_size(ge_handle h, int what);
 
 /* MujocoEnv.set_state + controller re-sync, as GraspEnv.reset_model does (GraspingEnv.py:466-470):

@@ -60,7 +60,7 @@ __device__ __forceinline__ int island_owner(const int* island, const int* tlist,
 
 __device__ __noinline__ void build_hessian(double* ws, int* wi, int ncon, int nsr, int lane) {
   const DevModel& m = c_m; const Layout& L = c_L;
-  double* H = ws + L.H;  // (CTA-per-env build: re-pointed at the env's HBM overflow row below if this build's blocks exceed L.hcap)
+  double* H = ws + L.H;  // (re-pointed at the env's HBM overflow row below if this build's blocks exceed L.hcap)
   const double *qM = ws + L.qM, *cdof = ws + L.cdof;
   const int wl = lane & 31, wid = lane >> 5;
   int* tcoupled = wi + L.i_tcoupled;
@@ -153,7 +153,6 @@ __device__ __noinline__ void build_hessian(double* ws, int* wi, int ncon, int ns
     }
     T_HOFF(tlist, t) = off;
   }
-#if GE_NW > 1
   {  // total size of this build's blocks (every thread adds up the same list)
     int tot = 0;
     for (int u = 0; u < m.ntree; u++) {
@@ -164,21 +163,25 @@ __device__ __noinline__ void build_hessian(double* ws, int* wi, int ncon, int ns
       tot += n * (n + 1) / 2;
     }
     const bool ovf = tot > L.hcap;
-    if (ovf) H = g_hovf;
+    if (ovf) H = g_hovf[threadIdx.y];
     if (lane == 0) {
       wi[L.i_hflag] = ovf ? 1 : 0;
-      // island -> warp: islands in descending order of size would be ideal; taking them in index order and always feeding the least
-      // loaded warp is within a small factor and needs no sort
-      long long load[GE_NW];
-      for (int w = 0; w < GE_NW; w++) load[w] = 0;
-      for (int u = 0; u < m.ntree; u++) {
-        if (!tcoupled[u] || island[u] != u) continue;
-        const long long n = tlist[u * GE_TLIST];
-        int best = 0;
-        for (int w = 1; w < GE_NW; w++) if (load[w] < load[best]) best = w;
-        load[best] += n * n * n + 64 * n * n;
-        tlist[u * GE_TLIST + 1] = best;
-      }
+      if (ovf) atomicAdd(L.hovf_builds, 1ULL);
+    }
+  }
+#if GE_NW > 1
+  if (lane == 0) {
+    // island -> warp: islands in descending order of size would be ideal; taking them in index order and always feeding the least
+    // loaded warp is within a small factor and needs no sort
+    long long load[GE_NW];
+    for (int w = 0; w < GE_NW; w++) load[w] = 0;
+    for (int u = 0; u < m.ntree; u++) {
+      if (!tcoupled[u] || island[u] != u) continue;
+      const long long n = tlist[u * GE_TLIST];
+      int best = 0;
+      for (int w = 1; w < GE_NW; w++) if (load[w] < load[best]) best = w;
+      load[best] += n * n * n + 64 * n * n;
+      tlist[u * GE_TLIST + 1] = best;
     }
   }
 #endif
@@ -418,10 +421,7 @@ __device__ __noinline__ bool mass_block_solve(double* ws, double* x, double hdam
 // own (island_owner) concurrently.
 __device__ __noinline__ void cholesky_solve(double* ws, int* wi, double* x, const double* g_, int lane) {
   const DevModel& m = c_m; const Layout& L = c_L;
-  double* H = ws + L.H;
-#if GE_NW > 1
-  if (wi[L.i_hflag]) H = g_hovf;
-#endif
+  double* H = wi[L.i_hflag] ? g_hovf[threadIdx.y] : ws + L.H;
   const int wl = lane & 31, wid = lane >> 5;
   const int *tcoupled = wi + L.i_tcoupled, *tlist = wi + L.i_tlist;
   bool any_coupled = false;

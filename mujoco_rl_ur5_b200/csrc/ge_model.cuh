@@ -57,10 +57,11 @@ struct Layout {
   int total_bytes;
   int maxcon, maxcand;          // capacity of the contact / candidate lists
   int fk_bytes;                 // bytes of the workspace prefix the kinematics stage touches (kinematics-only kernels)
-  int ws_global;                // 1: big-scene build (a CTA per env); E.gws then holds one overflow row per env for oversized Hessian builds
+  int ws_global;                // 1: big-scene build (a CTA per env)
   int hcap;                     // doubles of the Hessian block region at L.H (= nv (nv + 1) / 2 when everything always fits)
   int hfull;                    // nv (nv + 1) / 2: size of the overflow row
   int i_hflag;                  // int slot: 1 while the Hessian blocks of the current build live in the overflow row
+  unsigned long long* hovf_builds;  // [1] on the device: Hessian builds of this engine that used the overflow row (ge_size 13)
 };
 
 // per-environment state in HBM, row-major [N, ...]
@@ -81,5 +82,5 @@ struct EnvArrays {
   int* owed;                      // [N] visits of the env drawn in this launch and not yet run (k_run: a drawer never drops a visit)
   int* done;                      // [N] iterations the env has been given in this launch (reset before every launch)
   unsigned long long* ticket;     // [1] monotonically increasing task counter of k_run (never reset: launches subtract their base)
-  double* gws;                    // [N, hfull] Hessian overflow rows (big-scene build when hcap < hfull), else NULL
+  double* gws;                    // [N, hfull] Hessian overflow rows (when hcap < hfull), else NULL
 };

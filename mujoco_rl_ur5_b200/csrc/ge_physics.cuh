@@ -15,7 +15,10 @@ namespace ge {
 
 __constant__ DevModel c_m;
 __constant__ Layout c_L;
-__shared__ double* g_hovf;    // CTA-per-env build: HBM overflow row for the Hessian blocks of the env this CTA holds (may be null)
+// HBM overflow row for the Hessian blocks of the env each group of the CTA holds (may be null), indexed by threadIdx.y: one group per
+// CTA in the CTA-per-env build, up to GE_MAX_WPB warps in the warp-per-env build
+#define GE_MAX_WPB 16
+__shared__ double* g_hovf[GE_NW > 1 ? 1 : GE_MAX_WPB];
 __constant__ int c_nancheck;  // GE_NANCHECK=1: record in status bits 8.. the first pipeline stage that produced a non-finite value
 
 // Trip counts are data (items per lane, mostly 1 or 2): unrolling them only multiplies the code every warp has to fetch.

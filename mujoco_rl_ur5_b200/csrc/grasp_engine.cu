@@ -105,16 +105,20 @@ __device__ int env_take(const EnvArrays& E, int e, int nsub) {
 }
 // blockDim = (GE_LANES, envs per CTA): threadIdx.x is the lane inside the group that owns one environment (a warp; a whole CTA of
 // GE_NW warps in the big-scene build, where blockDim.y = 1)
-// Register budget.  Warp-per-env build: `__launch_bounds__(256)` alone makes ptxas settle on 128 registers per thread (stack 1616 B); told
-// that one 256-thread CTA per SM is enough it takes 246 (stack 1296 B), which still fits the 2 x 128-thread CTAs the shared memory allows
-// (65 536 registers per SM; -DGE_V0_CAP_REGS restores the 128-register budget).
+// Register budget.  Warp-per-env build: the workspace lets ten warps share an SM (ge_create), and the SM hands out registers per
+// quarter (16 384 each, in 256-register steps per warp): ten warps need three per quarter, i.e. <= 168 registers per thread.  Without a
+// cap ptxas takes 242 (2 warps per quarter = 8 per SM); `__maxnreg__(168)` costs a 1456 B stack (1296 B at 242) and small spills.
+// `__launch_bounds__(256)` alone gives 128 registers per thread (-DGE_V0_CAP_REGS); -DGE_RUN_MAXNREG=N tries another cap.
 // CTA-per-env build: two CTAs per SM is what the workspace allows; the bound keeps the register file from undercutting it.
 #if GE_NW > 1
 #define GE_RUN_BOUNDS __launch_bounds__(GE_LANES, 2)
 #elif defined(GE_V0_CAP_REGS)
 #define GE_RUN_BOUNDS __launch_bounds__(256)
 #else
-#define GE_RUN_BOUNDS __launch_bounds__(256, 1)
+#ifndef GE_RUN_MAXNREG
+#define GE_RUN_MAXNREG 168
+#endif
+#define GE_RUN_BOUNDS __maxnreg__(GE_RUN_MAXNREG)
 #endif
 __global__ void GE_RUN_BOUNDS k_run(EnvArrays E, int n_env, int nsub, int quota, unsigned long long ticket_base, double base_x, double base_y,
                                              double base_z, int stage_sync) {
@@ -151,7 +155,7 @@ __global__ void GE_RUN_BOUNDS k_run(EnvArrays E, int n_env, int nsub, int quota,
       if (!got) continue;
       env = e;
       __threadfence();
-      if (GE_NW > 1 && lane == 0) g_hovf = E.gws ? E.gws + (size_t)e * L.hfull : nullptr;  // this env's Hessian overflow row
+      if (lane == 0) g_hovf[threadIdx.y] = E.gws ? E.gws + (size_t)e * L.hfull : nullptr;  // this env's Hessian overflow row
     }
     if (env >= 0 && !running) {  // a visit was taken (drawn above, or owed to the env this group just stored): load and run it
       env_load(E, env, ws, lane, r);
@@ -224,7 +228,7 @@ __global__ void __launch_bounds__(GE_LANES) k_debug(EnvArrays E, int env, int fi
   const DevModel& m = c_m; const Layout& L = c_L;
   int lane = threadIdx.x;
   double* ws = smem;
-  if (GE_NW > 1 && threadIdx.x == 0) g_hovf = E.gws ? E.gws + (size_t)env * L.hfull : nullptr;
+  if (threadIdx.x == 0) g_hovf[0] = E.gws ? E.gws + (size_t)env * L.hfull : nullptr;
   int* wi = (int*)(ws + L.total_doubles);
   LANE_LOOP(i, m.nq) ws[L.qpos + i] = E.qpos[(size_t)env * m.nq + i];
   LANE_LOOP(i, m.nv) { ws[L.qvel + i] = E.qvel[(size_t)env * m.nv + i]; ws[L.qaccws + i] = E.qaccws[(size_t)env * m.nv + i]; }
@@ -273,7 +277,7 @@ __global__ void __launch_bounds__(GE_LANES) k_debug(EnvArrays E, int env, int fi
           else continue;
           tot += r * (r + 1) / 2;
         }
-        out[0] = GE_NW > 1 ? wi[L.i_hflag] : 0; out[1] = tot; out[2] = m.ntree;
+        out[0] = wi[L.i_hflag]; out[1] = tot; out[2] = m.ntree;
       }
       LANE_LOOP(t, (n <= cap ? m.ntree : 0)) {
         const bool c = tcoupled[t] != 0;
@@ -362,7 +366,7 @@ __global__ void __launch_bounds__(GE_LANES) k_step_open(EnvArrays E, int n_env, 
   int env = blockIdx.x, lane = threadIdx.x;
   if (env >= n_env || (emask && !emask[env])) return;
   double* ws = smem;
-  if (GE_NW > 1 && threadIdx.x == 0) g_hovf = E.gws ? E.gws + (size_t)env * L.hfull : nullptr;
+  if (threadIdx.x == 0) g_hovf[0] = E.gws ? E.gws + (size_t)env * L.hfull : nullptr;
   int* wi = (int*)(ws + L.total_doubles);
   LANE_LOOP(i, m.nq) ws[L.qpos + i] = E.qpos[(size_t)env * m.nq + i];
   LANE_LOOP(i, m.nv) { ws[L.qvel + i] = E.qvel[(size_t)env * m.nv + i]; ws[L.qaccws + i] = E.qaccws[(size_t)env * m.nv + i]; }
@@ -430,6 +434,7 @@ struct ge_engine {
   int stage_sync;    // CTA barriers between the stages of a sub-step (instruction-cache sharing)
   int quota;         // iterations per visit of k_run's dynamic env scheduling
   int max_ctas;      // resident CTAs of k_run on this device (persistent grid)
+  int groups_per_sm; // resident envs (groups) of k_run per SM that the occupancy API grants
   unsigned long long ticket_base;  // tasks issued by all previous launches
   int* d_nout; double* d_dbg;
   RenderCtx rctx;
@@ -461,23 +466,63 @@ static void make_layout(const DevModel& m, Layout& L, const int* tree_dofnum_h, 
   int nb = m.nbody, nj = m.njnt, nv = m.nv, ng = m.ngeom;
   int o = 0;
   auto take = [&](int n) { int r = o; o += align_up(n, 2); return r; };
+  // the tree-sparse L^T D L factor is only needed when a tree is too wide for the lane-group mass solve
+  bool need_ld = false;
+  for (int t = 0; t < ntree_dofnum_n; t++) if (tree_dofnum_h[t] > 8 && !tree_simple_h[t]) need_ld = true;
   L.qpos = take(m.nq); L.qvel = take(nv); L.qaccws = take(nv); L.ctl = take(32);
-  L.cdof = take(6 * nv); L.qM = take(m.nM);
-  {  // the tree-sparse L^T D L factor is only needed when a tree is too wide for the lane-group mass solve
-    bool need = false;
-    for (int t = 0; t < ntree_dofnum_n; t++) if (tree_dofnum_h[t] > 8 && !tree_simple_h[t]) need = true;
-    L.qLD = need ? take(m.nM) : L.qM;
-  }
-  L.qfrc_smooth = take(nv); L.qacc_smooth = take(nv); L.qfrc_constraint = take(nv); L.qacc = take(nv);
-  L.Ma = take(nv); L.grad = take(nv); L.search = take(nv); L.Mv = take(nv);
+  L.cdof = take(6 * nv);
   L.cstride = align_up(C_MU + 4 * m.maxdim - 1, 2);
-  // list capacities: the 6-object scene never exceeded 20 contacts; piles of free objects need room for ~3 contacts per object
   L.maxcon = maxcon;
   L.maxcand = 2 * L.maxcon;
+  L.hfull = nv * (nv + 1) / 2;
+  L.hcap = hcap > 0 && hcap < L.hfull ? hcap : L.hfull;
+  int end;
+#if GE_NW == 1
+  // Warp-per-env build: every array is placed by its lifetime inside one sub-step (ten envs share an SM only if the peak is small).
+  //   whole step:            state rows, cdof (fk -> Newton), contact list (collision -> Newton), qfrc_smooth (RNE -> Euler), qM (CRB -> Euler)
+  //   stage_fk only:         body poses and local joint frames, in the contact list's storage (dead before collision writes a contact)
+  //   fk -> CRB:             cinert; then the geom frames (fk -> collision), over which the RNE / CRB temporaries go
+  //   mass solve -> Euler:   the other dof vectors, simple rows, Vb and the Hessian region (which also holds nt_update's contact and
+  //                          body wrenches, dead while Hessian blocks are), over cinert and the RNE / CRB temporaries
+  L.con = take(L.maxcon * L.cstride);
+  L.qfrc_smooth = take(nv); L.qM = take(m.nM);
+  L.qLD = need_ld ? take(m.nM) : L.qM;
+  L.scratch = o;
+  int a = o;
+  auto takeA = [&](int n) { int r = a; a += align_up(n, 2); return r; };
+  L.cinert = takeA(10 * nb);
+  const int g0 = a;
+  L.gpos = takeA(3 * ng); L.gmat = takeA(9 * ng); L.gcen = takeA(3 * ng);
+  const int endG = a;
+  a = g0;
+  L.cdofdot = takeA(6 * nv); L.cvel = takeA(6 * nb); L.cacc = takeA(6 * nb); L.cfrc = takeA(6 * nb);  // crb (10 nb) goes over cvel + cacc
+  const int endT = a;
+  const int nfk = align_up(3 * nb, 2) + align_up(9 * nb, 2) + align_up(3 * nb, 2) + align_up(4 * nb, 2) + 2 * align_up(3 * nj, 2);
+  a = nfk <= L.maxcon * L.cstride ? L.con : (endG > endT ? endG : endT);
+  L.xpos = takeA(3 * nb); L.xmat = takeA(9 * nb); L.lpos = takeA(3 * nb); L.lquat = takeA(4 * nb); L.janchor = takeA(3 * nj); L.jaxis = takeA(3 * nj);
+  const int endF = a;
+  L.xquat = L.xpos; L.xipos = L.xpos;  // (not stored any more)
+  int b = L.scratch;
+  auto takeB = [&](int n) { int r = b; b += align_up(n, 2); return r; };
+  L.qacc_smooth = takeB(nv); L.qfrc_constraint = takeB(nv); L.qacc = takeB(nv);
+  L.sr = takeB(6 * GE_MAXSR);
+  L.Ma = takeB(nv); L.grad = takeB(nv); L.search = takeB(nv); L.Mv = takeB(nv);
+  L.Vb = takeB(6 * nb);
+  L.H = takeB(L.hcap);
+  L.Wb = L.hcap >= 6 * L.maxcon + 6 * nb ? L.H + 6 * L.maxcon : takeB(6 * nb);
+  end = endG;
+  for (int e : {endT, endF, b}) if (e > end) end = e;
+  L.fk_bytes = align_up(endG > endF ? endG : endF, 2) * 8;
+#else
+  // CTA-per-env build: fixed arrays, then one scratch region aliased by phase
+  L.qM = take(m.nM);
+  L.qLD = need_ld ? take(m.nM) : L.qM;
+  L.qfrc_smooth = take(nv); L.qacc_smooth = take(nv); L.qfrc_constraint = take(nv); L.qacc = take(nv);
+  L.Ma = take(nv); L.grad = take(nv); L.search = take(nv); L.Mv = take(nv);
+  // list capacities: the 6-object scene never exceeded 20 contacts; piles of free objects need room for ~3 contacts per object
   L.con = take(L.maxcon * L.cstride);
   L.sr = take(6 * GE_MAXSR);
   L.scratch = o;
-  // phase A (kinematics/dynamics/collision)
   // phase A (kinematics -> collision -> bias forces / mass matrix); order of use:
   //   stage_fk writes everything; stage_collision needs gpos/gmat/gcen only; stage_rne + stage_crb need cinert (+ their own
   //   temporaries, which overwrite the geom frames and body poses that are dead by then)
@@ -502,23 +547,23 @@ static void make_layout(const DevModel& m, Layout& L, const int* tree_dofnum_h, 
   // phase B (solver)
   int b = L.scratch;
   auto takeB = [&](int n) { int r = b; b += align_up(n, 2); return r; };
-  L.hfull = nv * (nv + 1) / 2;
-  L.hcap = hcap > 0 && hcap < L.hfull ? hcap : L.hfull;
   L.H = takeB(L.hcap); L.Vb = takeB(6 * nb); L.Wb = takeB(6 * nb);
   int endB = b;
   // crb (10*nb) is written over cvel+cacc (12*nb) — asserted by construction (cvel, cacc adjacent)
-  int end = endA1 > endA2 ? endA1 : endA2;
+  end = endA1 > endA2 ? endA1 : endA2;
   if (endB > end) end = endB;
-  L.total_doubles = align_up(end, 2);
   L.fk_bytes = align_up(endA1, 2) * 8;
+#endif
+  L.total_doubles = align_up(end, 2);
   int io = 0;
   auto takeI = [&](int n) { int r = io; io += n; return r; };
   L.i_cb1 = takeI(L.maxcon); L.i_cb2 = takeI(L.maxcon); L.i_ct1 = takeI(L.maxcon); L.i_ct2 = takeI(L.maxcon); L.i_cdim = takeI(L.maxcon); L.i_cpair = takeI(L.maxcon); L.i_cact = takeI(L.maxcon);
   L.i_srA = takeI(GE_MAXSR); L.i_srB = takeI(GE_MAXSR); L.i_srtype = takeI(GE_MAXSR); L.i_sract = takeI(GE_MAXSR);
-  L.i_cand = takeI(L.maxcand); L.i_first = takeI(nv); L.i_tcoupled = takeI(m.ntree); L.i_tcount = takeI(m.ntree); L.i_tlist = takeI(m.ntree * GE_TLIST); L.i_island = takeI(m.ntree); L.i_hflag = takeI(GE_NW > 1 ? 1 : 0);
+  L.i_cand = takeI(L.maxcand); L.i_first = takeI(nv); L.i_tcoupled = takeI(m.ntree); L.i_tcount = takeI(m.ntree); L.i_tlist = takeI(m.ntree * GE_TLIST); L.i_island = takeI(m.ntree); L.i_hflag = takeI(1);
   L.total_ints = align_up(io, 4);
   L.total_bytes = L.total_doubles * 8 + L.total_ints * 4;
   L.ws_global = 0;
+  L.hovf_builds = nullptr;
 }
 
 extern "C" int ge_create(const void* model_blob, size_t nbytes, int n_envs, int device, void* stream, ge_handle* out) {
@@ -584,9 +629,43 @@ extern "C" int ge_create(const void* model_blob, size_t nbytes, int n_envs, int 
   const int* tsi = (const int*)blob_find(B, "tree_simple", nullptr);
   // list capacities: the 6-object scene never exceeded 20 contacts; piles of free objects need room for ~3 contacts per object
   const int maxcon_default = m.ntree <= 8 ? 32 : 128;
+  int diag = 0;
+  for (int t = 0; t < m.ntree; t++) diag += tdn[t] * (tdn[t] + 1) / 2;
+  const int hfull = m.nv * (m.nv + 1) / 2;
+  cudaFuncAttributes run_attr;  // static shared memory of k_run (g_hovf, reduction slots) comes on top of the workspaces
+  CK(cudaFuncGetAttributes(&run_attr, k_run));
+  auto fit = [&](int maxcon, long budget) {
+    int lo = 0, hi = hfull;  // largest cap in [1, hfull] with total_bytes <= budget (0: none)
+    while (lo < hi) {
+      int mid = (lo + hi + 1) / 2;
+      Layout T;
+      make_layout(m, T, tdn, tsi, m.ntree, maxcon, mid);
+      if ((long)T.total_bytes <= budget) lo = mid; else hi = mid - 1;
+    }
+    return lo;
+  };
 #if GE_NW == 1
-  // warp-per-env build: the whole workspace (full Hessian triangle) in one shared-memory slice per warp, or not at all
-  make_layout(m, h->lay, tdn, tsi, m.ntree, maxcon_default, 0);
+  // warp-per-env build: one shared-memory slice per warp.  The Hessian region is capped so that ten envs share an SM (one CTA of ten
+  // warps or two of five: 10 slices + 2 x (static shared + 1 KB reserve) <= 228 KB); a Hessian build that needs more uses the env's
+  // overflow row in HBM.  The region must hold nt_update's contact and body wrenches, and the blocks of the mass solve (<= the tree
+  // diagonal).
+  {
+    const int maxcon = maxcon_default;
+    int need_min = 6 * maxcon + 6 * m.nbody;
+    if (diag > need_min) need_min = diag;
+    int cap = fit(maxcon, (233472 - 2 * (1024 + (long)run_attr.sharedSizeBytes)) / 10);
+    if (cap < need_min) cap = hfull;  // too large for ten per SM: the whole triangle, fewer envs per SM
+    make_layout(m, h->lay, tdn, tsi, m.ntree, maxcon, cap);
+    // GE_HCAP only moves the region of a scene this build holds anyway: a scene that needs the CTA-per-env build keeps it
+    if (const char* ev = getenv("GE_HCAP")) {
+      long v = atol(ev);
+      Layout T;
+      if (v >= need_min && v <= hfull && h->lay.total_bytes <= 227 * 1024) {
+        make_layout(m, T, tdn, tsi, m.ntree, maxcon, (int)v);
+        if (T.total_bytes <= 227 * 1024) h->lay = T;
+      }
+    }
+  }
   h->lay.ws_global = 0;
   if (h->lay.total_bytes > 227 * 1024) { cudaFree(h->dblob); delete h; return fail(GE_ERR_TOO_LARGE, "per-env workspace exceeds shared memory"); }
 #else
@@ -597,25 +676,12 @@ extern "C" int ge_create(const void* model_blob, size_t nbytes, int n_envs, int 
     // with an empty Hessian region - 3.3 KB over what lets two CTAs share an SM (settled piles hold 40-50 contacts; overflow is flagged)
     int maxcon = maxcon_default > 112 ? 112 : maxcon_default;
     if (const char* ev = getenv("GE_MAXCON")) { int v = atoi(ev); if (v >= 16 && v <= 512) maxcon = v; }
-    int diag = 0;
-    for (int t = 0; t < m.ntree; t++) diag += tdn[t] * (tdn[t] + 1) / 2;
-    const int hfull = m.nv * (m.nv + 1) / 2;
     int need_min = diag + 6 * maxcon + 64;  // all trees uncoupled / the contact-wrench scratch of nt_update
     if (need_min > hfull) need_min = hfull;
     // the Hessian region shares the phase-aliased scratch with the kinematics arrays: largest cap whose layout fits the budget
-    auto fit = [&](long budget) {
-      int lo = 0, hi = hfull;  // largest cap in [1, hfull] with total_bytes <= budget (0: none)
-      while (lo < hi) {
-        int mid = (lo + hi + 1) / 2;
-        Layout T;
-        make_layout(m, T, tdn, tsi, m.ntree, maxcon, mid);
-        if ((long)T.total_bytes <= budget) lo = mid; else hi = mid - 1;
-      }
-      return lo;
-    };
     const long budget2 = 233472 / 2 - 1024 - 2048, budget1 = 227 * 1024 - 2048;  // per CTA: system reserve and the static arrays taken off
-    int cap = fit(budget2);
-    if (cap < need_min) cap = fit(budget1);
+    int cap = fit(maxcon, budget2);
+    if (cap < need_min) cap = fit(maxcon, budget1);
     if (cap < need_min) { cudaFree(h->dblob); delete h; return fail(GE_ERR_MODEL, "model too large: per-env workspace exceeds shared memory even with one CTA per SM"); }
     if (const char* ev = getenv("GE_HCAP")) { long v = atol(ev); if (v >= need_min && v <= hfull) cap = (int)v; }
     make_layout(m, h->lay, tdn, tsi, m.ntree, maxcon, cap);
@@ -624,20 +690,23 @@ extern "C" int ge_create(const void* model_blob, size_t nbytes, int n_envs, int 
   }
 #endif
   if (h->lay.fk_bytes > 227 * 1024) { cudaFree(h->dblob); delete h; return fail(GE_ERR_MODEL, "model too large: kinematics workspace exceeds shared memory"); }
+  CK(cudaMalloc(&h->lay.hovf_builds, sizeof(unsigned long long)));
+  CK(cudaMemset(h->lay.hovf_builds, 0, sizeof(unsigned long long)));
   CK(cudaMemcpyToSymbol(c_m, &m, sizeof m));
   CK(cudaMemcpyToSymbol(c_L, &h->lay, sizeof(Layout)));
   { int nc = 0; if (const char* ev = getenv("GE_NANCHECK")) nc = atoi(ev) != 0; CK(cudaMemcpyToSymbol(c_nancheck, &nc, sizeof nc)); }
-  // warps (= envs) per CTA: maximise the resident warps per SM (228 KB shared memory per SM, 1 KB reserved per CTA, 227 KB max per
-  // CTA); ties go to the smaller CTA (less barrier imbalance).  r01 sweeps are in DESIGN.md; GE_WPB overrides.
+  // warps (= envs) per CTA: the most resident warps per SM as the occupancy API counts them (shared memory, and registers, which the
+  // SM allocates per sub-partition: four quarters of 16 384, so 200 registers per thread allow 2 warps per quarter and 168 allow 3);
+  // ties go to the larger CTA, whose warps walk the stage code together (DESIGN.md section 4).  GE_WPB overrides.
+  CK(cudaFuncSetAttribute(k_run, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024 - (int)run_attr.sharedSizeBytes));
   if (GE_NW > 1) h->wpb = 1;  // CTA-per-env build: one environment per CTA of GE_NW warps
   else {
     int best = 1, best_warps = 0;
-    for (int w = 1; w <= 8; w++) {
-      long per_cta = (long)w * h->lay.total_bytes;
-      if (per_cta > 227 * 1024) break;
-      int ctas = (int)(233472 / (per_cta + 1024));
-      if (ctas > 32) ctas = 32;
-      if (w * ctas > best_warps) { best_warps = w * ctas; best = w; }
+    for (int w = 1; w <= GE_MAX_WPB; w++) {
+      if ((long)w * h->lay.total_bytes + run_attr.sharedSizeBytes > 227 * 1024) break;
+      int ctas = 0;
+      CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctas, k_run, GE_LANES * w, (size_t)w * h->lay.total_bytes));
+      if (w * ctas >= best_warps) { best_warps = w * ctas; best = w; }
     }
     h->wpb = best;
   }
@@ -645,17 +714,14 @@ extern "C" int ge_create(const void* model_blob, size_t nbytes, int n_envs, int 
   if (const char* ev = getenv("GE_STAGE_SYNC")) h->stage_sync = atoi(ev) != 0;
   if (GE_NW > 1) h->stage_sync = 0;
   if (const char* ev = getenv("GE_DBG_NOSTEP")) if (atoi(ev) != 0) h->stage_sync |= 0x100;
-  if (const char* ev = getenv("GE_WPB")) if (GE_NW == 1) { int v = atoi(ev); if (v >= 1 && v <= 8 && v * h->lay.total_bytes <= 227 * 1024) h->wpb = v; }
+  if (const char* ev = getenv("GE_WPB")) if (GE_NW == 1) { int v = atoi(ev); if (v >= 1 && v <= GE_MAX_WPB && v * h->lay.total_bytes <= 227 * 1024) h->wpb = v; }
   h->ws_smem = (size_t)h->lay.total_bytes;
   if (getenv("GE_VERBOSE"))
     fprintf(stderr, "grasp_engine: %s build, workspace %d B per env (%d doubles + %d ints), contacts <= %d, Hessian region %d of %d doubles, %d env(s) per CTA\n",
             GE_NW > 1 ? "CTA-per-env" : "warp-per-env", h->lay.total_bytes, h->lay.total_doubles, h->lay.total_ints, h->lay.maxcon, h->lay.hcap, h->lay.hfull, h->wpb);
-  if (h->ws_smem) {
-    CK(cudaFuncSetAttribute(k_run, cudaFuncAttributeMaxDynamicSharedMemorySize, h->wpb * h->lay.total_bytes));
-    if (h->lay.total_bytes > 48 * 1024) {
-      CK(cudaFuncSetAttribute(k_debug, cudaFuncAttributeMaxDynamicSharedMemorySize, h->lay.total_bytes));
-      CK(cudaFuncSetAttribute(k_step_open, cudaFuncAttributeMaxDynamicSharedMemorySize, h->lay.total_bytes));
-    }
+  if (h->ws_smem && h->lay.total_bytes > 48 * 1024) {
+    CK(cudaFuncSetAttribute(k_debug, cudaFuncAttributeMaxDynamicSharedMemorySize, h->lay.total_bytes));
+    CK(cudaFuncSetAttribute(k_step_open, cudaFuncAttributeMaxDynamicSharedMemorySize, h->lay.total_bytes));
   }
   if (h->lay.fk_bytes > 48 * 1024) CK(cudaFuncSetAttribute(k_body_xpos, cudaFuncAttributeMaxDynamicSharedMemorySize, h->lay.fk_bytes));
   EnvArrays& E = h->E;
@@ -674,6 +740,7 @@ extern "C" int ge_create(const void* model_blob, size_t nbytes, int n_envs, int 
     CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_run, GE_LANES * h->wpb, (size_t)h->wpb * h->ws_smem));
     CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
     h->max_ctas = per_sm * sms > 0 ? per_sm * sms : 1;
+    h->groups_per_sm = per_sm * h->wpb;
     if (const char* ev = getenv("GE_MAXCTAS")) { int v = atoi(ev); if (v >= 1 && v < h->max_ctas) h->max_ctas = v; }  // experiments: fewer resident CTAs
   }
   E.gws = nullptr;
@@ -708,7 +775,7 @@ extern "C" int ge_destroy(ge_handle h) {
   EnvArrays& E = h->E;
   void* ptrs[] = {E.qpos, E.qvel, E.qaccws, E.ctl, E.cmd_mask, E.cmd_maxsteps, E.cmd_steps, E.cmd_result, E.cmd_active, E.cmd_tol, E.prog_phase,
                   E.prog_rot, E.prog_grasp, E.prog_aux, E.prog_info, E.prog_coords, E.prog_table, E.reward, E.status, E.substeps, E.busy_count,
-                  h->d_nout, h->d_dbg, h->dblob, E.gws, E.lock, E.owed, E.done, E.ticket};
+                  h->d_nout, h->d_dbg, h->dblob, E.gws, E.lock, E.owed, E.done, E.ticket, h->lay.hovf_builds};
   for (void* p : ptrs) cudaFree(p);
   render_free(h->rctx);
   delete h;
@@ -720,7 +787,14 @@ extern "C" int ge_size(ge_handle h, int what) {
   switch (what) {
     case 0: return h->hm.nq; case 1: return h->hm.nv; case 2: return h->hm.nbody; case 3: return h->hm.ngeom; case 4: return h->hm.nu;
     case 5: return h->n_envs; case 6: return h->lay.maxcon; case 7: return h->lay.total_bytes; case 8: return h->wpb; case 9: return h->lay.ws_global;
-    case 10: return h->lay.hcap; case 11: return h->lay.hfull;
+    case 10: return h->lay.hcap; case 11: return h->lay.hfull; case 12: return h->groups_per_sm;
+    case 13: {  // Hessian builds that used the overflow row since ge_create (saturates at INT_MAX)
+      unsigned long long n = 0;
+      CK(cudaSetDevice(h->device));
+      CK(cudaStreamSynchronize(h->stream));
+      CK(cudaMemcpy(&n, h->lay.hovf_builds, sizeof n, cudaMemcpyDeviceToHost));
+      return n > 0x7fffffffULL ? 0x7fffffff : (int)n;
+    }
   }
   return GE_ERR_ARG;
 }

@@ -97,7 +97,8 @@ class BatchedEngine:
     def size(self, what):
         """ge_size: 0 nq, 1 nv, 2 nbody, 3 ngeom, 4 nu, 5 n_envs, 6 max contacts, 7 workspace bytes per env, 8 envs per CTA,
         9 workspace placement (0 shared memory, 1 HBM rows), 10 doubles of the Newton Hessian block region in the workspace (hcap),
-        11 doubles of a full packed Hessian = of one env's HBM overflow row (hfull)"""
+        11 doubles of a full packed Hessian = of one env's HBM overflow row (hfull), 12 envs of the sub-step kernel resident per SM
+        (occupancy API), 13 Newton Hessian builds that used the overflow row since creation"""
         return int(self.L.ge_size(self.h, int(what)))
 
     # ------------------------------------------------------------------ helpers

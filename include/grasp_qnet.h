@@ -113,6 +113,12 @@ int gq_bn_running_update(const float* merged_stats, float* running_mean, float* 
  * As in torch's fp32 autograd, an image whose q_pred is exactly 0 or 1 contributes loss 100 (or 0) and no gradient. */
 int gq_loss_head_bwd(const float* q, const void* x, const float* w_head, const long long* action, const float* reward, int B, int A, int H, int W,
                      float* loss_terms, float* qsel, void* dX, float* dW_partial, float* db_partial, float* dW_head, float* db_head, void* stream);
+/* The same with importance weights weight [B] f32 (prioritized replay): loss = mean(w_b loss_b) = binary_cross_entropy(q_pred, reward,
+ * weight=w), loss_terms[b] = w_b loss_b and the gradient of image b scaled by w_b.  With every w_b = 1 the outputs equal gq_loss_head_bwd's
+ * bit for bit. */
+int gq_loss_head_bwd_weighted(const float* q, const void* x, const float* w_head, const long long* action, const float* reward, const float* weight, int B,
+                              int A, int H, int W, float* loss_terms, float* qsel, void* dX, float* dW_partial, float* db_partial, float* dW_head,
+                              float* db_head, void* stream);
 /* backward of y = relu(BatchNorm(o) [+ identity]) with batch statistics (BasicBlock, Modules.py:128-142): dY, act = y [B,HW,C] bf16, o [B,HW,C] f32,
  * stats merged [B,C,2], gamma [C].  Out: d_o [B,HW,C] bf16 (gradient w.r.t. the convolution output), dgamma, dbeta [C] (either may be NULL),
  * dpre_out (NULL or [B,HW,C] bf16) = dY * (y > 0), the gradient that also enters the identity branch.
@@ -133,6 +139,22 @@ int gq_upsample2x_bwd(const void* dY, void* dX, int B, int H, int W, int C, void
 int gq_add_to_bf16(const float* a, const float* b, const void* c_bf16, void* out, size_t n, void* stream);
 /* torch.optim.Adam step with weight_decay as L2 (Grasping_Agent_multidiscrete.py:153-156): p, g, m, v [n] f32, step counted from 1 */
 int gq_adam(float* p, const float* g, float* m, float* v, size_t n, float lr, float beta1, float beta2, float eps, float weight_decay, int step, void* stream);
+
+/* ------------------------------------------------------------------------------------------------------------------------------------
+ * Prioritized experience replay (Schaul et al. 2016, proportional) - see csrc/qnet_replay.cuh.  tree [2 cap] f64: an implicit sum-tree,
+ * cap = the smallest power of two >= the replay size (at most 2^30), slot i = leaf cap + i, node k = tree[2k] + tree[2k+1], root
+ * tree[1]; zero-initialised by the caller.  pmax [1] f64 = the largest priority ever assigned, 1.0 initially. */
+/* new transitions: leaves of slot [n] int64 (distinct, < cap) := pmax, ancestors recomputed */
+int gq_per_push(double* tree, const double* pmax, const long long* slot, int n, int cap, void* stream);
+/* stratified proportional sampling of B <= 1024 slots: stratum j draws U from Philox4x32-10 (counter (0xC0000000 + j, update_lo, update_hi,
+ * rank), key (seed_lo, seed_hi)), u = (j + U) total / B, and descends from the root (right iff u >= left and the right sum > 0).
+ * length = slots filled (the N of the weights).  Out: idx_out [B] int64, weight_out [B] f32 = (length p_j / total)^-beta / max_j(...) */
+int gq_per_sample(const double* tree, int cap, long long length, int B, double beta, unsigned long long seed, unsigned long long update, unsigned int rank,
+                  long long* idx_out, float* weight_out, void* stream);
+/* priorities of a trained batch: p_j = (|reward_j - qsel_j| + eps)^alpha, applied in batch order (a slot drawn twice keeps the later value),
+ * ancestors recomputed, pmax raised.  idx [B] int64 (B <= 1024), qsel / reward [B] f32 */
+int gq_per_update(double* tree, double* pmax, const long long* idx, const float* qsel, const float* reward, int B, double alpha, double eps, int cap,
+                  void* stream);
 
 #ifdef __cplusplus
 }

@@ -15,6 +15,11 @@ its keyed step counter is the number of the batch's first transition.  Checkpoin
 Cost: updates_per_step defaults to n_envs, the reference's one learn() per transition.  A learn() step of batch 12 is a forward and
 backward of the whole network, so at that ratio the learner dominates a batched step; DESIGN.md section 5 gives measured times.
 
+Prioritized replay (`prioritized=dict(alpha, beta0, beta_updates, eps)`, off by default): the replay is a
+PrioritizedObservationReplay, every update draws its batch in proportion to the priorities, keyed on (seed, learner update, rank),
+trains on the importance-weighted loss with beta going linearly from beta0 to 1 over beta_updates updates, and writes the batch's new
+priorities (|r - q_pred| + eps)^alpha back.  Without it the trainer is the reference's uniform rule, unchanged.
+
 Multi-GPU (torchrun): rank r runs envs [r N, (r + 1) N) of N_total = world N, the learner all-reduces its gradients over the process
 group, each rank keeps its own replay and sampling stream random.Random(seed + rank), the counters are summed when a checkpoint is
 written and rank 0 writes it.
@@ -30,10 +35,18 @@ import numpy as np
 
 from .batched_env import BatchedGraspEnv
 from .qnet_learn import QNetLearner
-from .replay_buffer import ObservationReplay
+from .replay_buffer import ObservationReplay, PrioritizedObservationReplay
 
 EPS_START, EPS_END, EPS_DECAY = 1.0, 0.2, 8000   # Grasping_Agent_multidiscrete.py:35-37
 COUNTERS = ("greedy_rotations", "greedy_rotations_successes", "random_rotations_successes")
+PER_DEFAULTS = dict(alpha=0.6, beta0=0.4, eps=1e-6)  # Schaul et al. 2016, proportional variant; beta_updates has no default
+
+
+def per_beta(update, beta0, beta_updates):
+    """importance-sampling exponent of learner update `update` (0-based): linear from beta0 at update 0 to 1 at beta_updates, then 1"""
+    if beta_updates <= 0:
+        return 1.0
+    return beta0 + (1.0 - beta0) * min(1.0, update / beta_updates)
 
 
 def epsilon(n, eps_start=EPS_START, eps_end=EPS_END, eps_decay=EPS_DECAY):
@@ -52,7 +65,7 @@ def load_checkpoint(path_or_dict):
 class BatchedTrainer:
     def __init__(self, n_envs, scene="A", device=0, seed=0, batch_size=12, mem_size=None, updates_per_step=None, lr=1e-3, eps_start=EPS_START,
                  eps_end=EPS_END, eps_decay=EPS_DECAY, load=None, env_index_offset=None, n_total=None, process_group=None, chunk=64, max_draws=256,
-                 noise_std=0.001, log=None):
+                 noise_std=0.001, log=None, prioritized=None):
         import torch
         import torch.distributed as dist
 
@@ -85,7 +98,15 @@ class BatchedTrainer:
         self.run_counts = np.zeros((len(COUNTERS), len(self.env.rotations)), dtype=np.int64)
         mem = max(2000, 4 * self.n_envs) if mem_size is None else int(mem_size)
         W, H = self.env.IMAGE_WIDTH, self.env.IMAGE_HEIGHT
-        self.replay = ObservationReplay(mem, (H, W), device=self.dev, rng=random.Random(self.seed + rank))
+        self.per = None
+        if prioritized is None:
+            self.replay = ObservationReplay(mem, (H, W), device=self.dev, rng=random.Random(self.seed + rank))
+        else:
+            unknown = set(prioritized) - set(PER_DEFAULTS) - {"beta_updates"}
+            if unknown or "beta_updates" not in prioritized:
+                raise ValueError(f"prioritized takes alpha, beta0, beta_updates (required) and eps; got {sorted(prioritized)}")
+            self.per = {**PER_DEFAULTS, **prioritized}
+            self.replay = PrioritizedObservationReplay(mem, (H, W), device=self.dev, alpha=self.per["alpha"], eps=self.per["eps"])
         A = self.env.arrays
         cam = self.env.cam
         self.camera = (float(np.asarray(A["cam_fovy"]).ravel()[cam]), np.asarray(A["cam_pos0"], dtype=np.float64).reshape(-1, 3)[cam],
@@ -151,8 +172,11 @@ class BatchedTrainer:
         losses = []
         if len(self.replay) >= 2 * self.batch_size:  # :396-399
             for _ in range(self.updates_per_step):
-                s, a, r = self.replay.sample(self.batch_size, self.learner.fw, self.seed, self.depth_threshold, self.noise_std)
-                losses.append(self.learner.learn_step(s, a, r))
+                if self.per is None:
+                    s, a, r = self.replay.sample(self.batch_size, self.learner.fw, self.seed, self.depth_threshold, self.noise_std)
+                    losses.append(self.learner.learn_step(s, a, r))
+                else:
+                    losses.append(self.prioritized_update())
         mark("learn")
         # update_tensorboard's counters (:448-466), keyed by str(rotation) like the reference's defaultdicts
         rot = act[:, 1].cpu().numpy()
@@ -174,6 +198,16 @@ class BatchedTrainer:
             self.log.write(json.dumps(rec) + "\n")
             self.log.flush()
         return rec
+
+    def prioritized_update(self):
+        """one learner update on a prioritized batch: draw (keyed on the learner's update count and this rank), weighted learn step,
+        new priorities of the drawn slots.  -> the weighted loss"""
+        u = self.learner.step_count
+        beta = per_beta(u, self.per["beta0"], self.per["beta_updates"])
+        s, a, r, idx, w = self.replay.sample(self.batch_size, self.learner.fw, self.seed, beta, u, self.rank, self.depth_threshold, self.noise_std)
+        loss, qsel = self.learner.learn_step(s, a, r, return_pred=True, weight=w)
+        self.replay.update_priorities(idx, qsel, r)
+        return loss
 
     def train(self, episodes, steps_per_episode):
         for _ in range(episodes):
@@ -234,6 +268,9 @@ def main(argv=None):
     p.add_argument("--seed", type=int, default=0)
     p.add_argument("--load", default=None, help="checkpoint to resume from (the reference's or this trainer's)")
     p.add_argument("--out", default=None, help="checkpoint written at the end")
+    p.add_argument("--prioritized", action="store_true", help="prioritized experience replay (proportional); beta reaches 1 after the number of updates this run plans")
+    p.add_argument("--per-alpha", type=float, default=PER_DEFAULTS["alpha"], help="priority exponent (with --prioritized)")
+    p.add_argument("--per-beta0", type=float, default=PER_DEFAULTS["beta0"], help="initial importance-sampling exponent (with --prioritized)")
     a = p.parse_args(argv)
     import os
 
@@ -246,9 +283,13 @@ def main(argv=None):
         torch.cuda.set_device(device)
         dist.init_process_group("nccl")
         pg = dist.group.WORLD
+    per = None
+    if a.prioritized:
+        planned = a.episodes * a.steps_per_episode * (a.envs if a.updates_per_step is None else a.updates_per_step)
+        per = dict(alpha=a.per_alpha, beta0=a.per_beta0, beta_updates=planned)
     tr = BatchedTrainer(a.envs, a.scene, device, seed=a.seed, batch_size=a.batch_size, mem_size=a.mem_size, updates_per_step=a.updates_per_step, lr=a.lr,
                         eps_start=a.eps_start, eps_end=a.eps_end, eps_decay=a.eps_decay, load=a.load, process_group=pg,
-                        log=sys.stdout if (pg is None or dist.get_rank() == 0) else None)
+                        log=sys.stdout if (pg is None or dist.get_rank() == 0) else None, prioritized=per)
     try:
         tr.train(a.episodes, a.steps_per_episode)
         if a.out:

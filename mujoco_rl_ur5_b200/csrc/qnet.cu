@@ -572,6 +572,9 @@ __device__ __forceinline__ void jitter_op(int op, float f, float mean, float& r,
 //   j = 1      w0 -> hue factor; w1 -> operation order = permutation number (uint64)w1 * 24 >> 32 of (0,1,2,3), permutations in
 //              lexicographic order (0 = 0123, 1 = 0132, ..., 23 = 3210)
 //   j = 2 + k  w0 -> k-th random-action candidate (uint64)w0 * (W*H*R) >> 32 (flat action rot*W*H + y*W + x)
+// Prioritized replay (qnet_replay.cuh) draws in its own domain c0 = 0xC0000000 + j, above both of these, with counter
+// (c0, update_lo, update_hi, rank): the learner update and the process rank take the place of the env and the step.
+//   j < B      w0, w1 -> stratum j's uniform U = ((w0 >> 5) 2^26 + (w1 >> 6)) 2^-53 in double (53 bits)
 // Uniforms are ((w >> 8) + 0.5) / 2^24 in float, as in obs_noise; factors 0.5 + u (brightness, contrast, saturation: 1 +- 0.5) and
 // u - 0.5 (hue: +-0.5), the ranges of ColorJitter(0.5, 0.5, 0.5, 0.5).  tests/test_batched_train.py restates this table in numpy.
 #define KEYED_C0 0x80000000u
@@ -974,3 +977,4 @@ extern "C" int gq_argmax(const float* q, int B, int n, int* idx, float* val, voi
   return 0;
 }
 #include "qnet_learn.cuh"
+#include "qnet_replay.cuh"

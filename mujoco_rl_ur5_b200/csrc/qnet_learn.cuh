@@ -51,21 +51,25 @@ __global__ void k_bn_running_update(const float* __restrict__ stats, float* __re
 //   dx[pix,:] += g w W_head[rot,:],  dW_head[rot,:] += g w x[pix,:],  db_head[rot] += g w.
 // Outputs: loss_terms [B] (-(r log q + (1-r) log(1-q)), logs clamped at -100 like torch), dX [B,H,W,64] bf16 (zero-filled by the
 // caller, 4 rows written here), dWp [B,A,64] / dbp [B,A] per-image partials (zero except row rot), qsel [B] the gathered q.
+// weight [B] (NULL: every w_b = 1, the unweighted loss bit for bit): importance weights of prioritized replay, the loss
+// mean(w_b loss_b) = binary_cross_entropy(q, r, weight=w); loss_terms[b] and the gradient of image b are scaled by w_b.
 __global__ void __launch_bounds__(64) k_loss_head_bwd(const float* __restrict__ q, const bf16* __restrict__ x, const float* __restrict__ w_head,
-                                                     const long long* __restrict__ action, const float* __restrict__ reward, int B, int A, int H, int W,
-                                                     float* __restrict__ loss_terms, float* __restrict__ qsel, bf16* __restrict__ dX, float* __restrict__ dWp,
+                                                     const long long* __restrict__ action, const float* __restrict__ reward, const float* __restrict__ weight,
+                                                     int B, int A, int H, int W, float* __restrict__ loss_terms, float* __restrict__ qsel, bf16* __restrict__ dX, float* __restrict__ dWp,
                                                      float* __restrict__ dbp) {
   const int b = blockIdx.x, c = threadIdx.x;  // thread = head input channel
   const int OH = 2 * H, OW = 2 * W;
   const long long a = action[b];
   const int rot = (int)(a / ((long long)OH * OW)), oy = (int)((a / OW) % OH), ox = (int)(a % OW);
   const float qv = q[(((size_t)b * A + rot) * OH + oy) * OW + ox], r = reward[b];
+  const float wb = weight ? weight[b] : 1.f;
   if (c == 0) {
-    loss_terms[b] = -(r * fmaxf(logf(qv), -100.f) + (1.f - r) * fmaxf(logf(1.f - qv), -100.f));
+    const float term = -(r * fmaxf(logf(qv), -100.f) + (1.f - r) * fmaxf(logf(1.f - qv), -100.f));
+    loss_terms[b] = weight ? wb * term : term;
     qsel[b] = qv;
   }
   const float sg = (1.f - qv) * qv;
-  const float g = (1.f / (float)B) * (qv - r) / fmaxf(sg, 1e-12f) * sg;
+  const float g = (wb / (float)B) * (qv - r) / fmaxf(sg, 1e-12f) * sg;
   const float fy = oy * (float)(H - 1) / (float)(OH - 1), fx = ox * (float)(W - 1) / (float)(OW - 1);
   const int y0 = (int)fy, x0 = (int)fx, y1 = min(y0 + 1, H - 1), x1 = min(x0 + 1, W - 1);
   const float wy = fy - y0, wx = fx - x0;
@@ -452,19 +456,31 @@ extern "C" int gq_bn_running_update(const float* merged_stats, float* running_me
   QCK(cudaGetLastError());
   return 0;
 }
-extern "C" int gq_loss_head_bwd(const float* q, const void* x, const float* w_head, const long long* action, const float* reward, int B, int A, int H, int W,
-                                float* loss_terms, float* qsel, void* dX, float* dW_partial, float* db_partial, float* dW_head, float* db_head, void* stream) {
+static int loss_head_bwd(const char* what, const float* q, const void* x, const float* w_head, const long long* action, const float* reward, const float* weight,
+                         int B, int A, int H, int W, float* loss_terms, float* qsel, void* dX, float* dW_partial, float* db_partial, float* dW_head, float* db_head,
+                         void* stream) {
   if (!q || !x || !w_head || !action || !reward || !loss_terms || !qsel || !dX || !dW_partial || !db_partial || !dW_head || !db_head || A > 64) {
-    snprintf(q_err, sizeof q_err, "gq_loss_head_bwd: bad argument");
+    snprintf(q_err, sizeof q_err, "%s: bad argument", what);
     return -1;
   }
   cudaStream_t st = (cudaStream_t)stream;
   QCK(cudaMemsetAsync(dX, 0, (size_t)B * H * W * 64 * sizeof(bf16), st));
-  k_loss_head_bwd<<<B, 64, 0, st>>>(q, (const bf16*)x, w_head, action, reward, B, A, H, W, loss_terms, qsel, (bf16*)dX, dW_partial, db_partial);
+  k_loss_head_bwd<<<B, 64, 0, st>>>(q, (const bf16*)x, w_head, action, reward, weight, B, A, H, W, loss_terms, qsel, (bf16*)dX, dW_partial, db_partial);
   k_reduce_rows<<<(A * 64 + 127) / 128, 128, 0, st>>>(dW_partial, dW_head, B, (size_t)A * 64);
   k_reduce_rows<<<1, 128, 0, st>>>(db_partial, db_head, B, (size_t)A);
   QCK(cudaGetLastError());
   return 0;
+}
+extern "C" int gq_loss_head_bwd(const float* q, const void* x, const float* w_head, const long long* action, const float* reward, int B, int A, int H, int W,
+                                float* loss_terms, float* qsel, void* dX, float* dW_partial, float* db_partial, float* dW_head, float* db_head, void* stream) {
+  return loss_head_bwd("gq_loss_head_bwd", q, x, w_head, action, reward, nullptr, B, A, H, W, loss_terms, qsel, dX, dW_partial, db_partial, dW_head, db_head, stream);
+}
+extern "C" int gq_loss_head_bwd_weighted(const float* q, const void* x, const float* w_head, const long long* action, const float* reward, const float* weight,
+                                         int B, int A, int H, int W, float* loss_terms, float* qsel, void* dX, float* dW_partial, float* db_partial, float* dW_head,
+                                         float* db_head, void* stream) {
+  if (!weight) { snprintf(q_err, sizeof q_err, "gq_loss_head_bwd_weighted: bad argument"); return -1; }
+  return loss_head_bwd("gq_loss_head_bwd_weighted", q, x, w_head, action, reward, weight, B, A, H, W, loss_terms, qsel, dX, dW_partial, db_partial, dW_head,
+                       db_head, stream);
 }
 extern "C" int gq_bn_relu_bwd(const void* dY, const void* act, const float* o, const float* stats, const float* gamma, int B, int HW, int C, float eps,
                               void* dpre_out, float* scratch_part, float* scratch_sums, float* dgamma, float* dbeta, void* d_o, void* stream) {

@@ -105,12 +105,17 @@ def _bind_learn(L):
     L.gq_add_to_bf16.argtypes = [P, P, P, P, C.c_size_t, P]
     L.gq_adam.argtypes = [P, P, P, P, C.c_size_t, F, F, F, F, F, I, P]
     L.gq_bn_running_update.argtypes = [P, P, P, I, I, I, F, P]
+    L.gq_loss_head_bwd_weighted.argtypes = [P, P, P, P, P, P, I, I, I, I, P, P, P, P, P, P, P, P]
+    D, U64 = C.c_double, C.c_uint64
+    L.gq_per_push.argtypes = [P, P, P, I, I, P]
+    L.gq_per_sample.argtypes = [P, I, C.c_longlong, I, D, U64, U64, C.c_uint32, P, P, P]
+    L.gq_per_update.argtypes = [P, P, P, P, P, I, D, D, I, P]
     L._learn_bound = True
     return L
 
 
 LEARN_SYMBOLS = ["gq_bn_batch_merge", "gq_loss_head_bwd", "gq_bn_relu_bwd", "gq_conv_wgrad", "gq_conv_first_wgrad", "gq_maxpool_bwd", "gq_upsample2x_bwd",
-                 "gq_add_to_bf16", "gq_adam", "gq_bn_running_update"]
+                 "gq_add_to_bf16", "gq_adam", "gq_bn_running_update", "gq_loss_head_bwd_weighted", "gq_per_push", "gq_per_sample", "gq_per_update"]
 
 
 class QNetLearner:
@@ -347,10 +352,11 @@ class QNetLearner:
         assert idx and idx == list(range(idx[0], idx[-1] + 1)), prefix
         return self.grad[int(self.offsets[idx[0]]):int(self.offsets[idx[-1] + 1])]
 
-    def backward(self, q, saved, action, reward, on_ready=None):
+    def backward(self, q, saved, action, reward, on_ready=None, weight=None):
         """-> loss (0-dim tensor), q_pred [B]; fills self.grad (every parameter gradient of the step).  `on_ready(prefix)` is called as
         soon as all gradients of one parameter group (a BasicBlock, the head, the first convolution) have been enqueued - the
-        multi-GPU learner starts that group's all-reduce there, under the rest of the backward pass."""
+        multi-GPU learner starts that group's all-reduce there, under the rest of the backward pass.  weight [B] f32 on the device
+        (prioritized replay's importance weights): the loss is binary_cross_entropy(q_pred, reward, weight=weight)."""
         ready = on_ready if on_ready is not None else (lambda prefix: None)
         t, fw = self.torch, self.fw
         B, H, W, h, w, h2, w2 = saved["dims"]
@@ -363,9 +369,15 @@ class QNetLearner:
         dWp = t.empty((B, A, 64), dtype=t.float32, device=self.dev)
         dbp = t.empty((B, A), dtype=t.float32, device=self.dev)
         dW_head = t.empty((A, 64), dtype=t.float32, device=self.dev)
-        self._ck(self.L.gq_loss_head_bwd(self._p(q), self._p(saved["b5"]), self._p(fw.w_head), self._p(action), self._p(reward), B, A, 2 * h2, 2 * w2,
-                                         self._p(loss_terms), self._p(qsel), self._p(d_b5), self._p(dWp), self._p(dbp), self._p(dW_head), self._p(self.g["1.C1.bias"]),
-                                         self._st()), "gq_loss_head_bwd")
+        if weight is None:
+            self._ck(self.L.gq_loss_head_bwd(self._p(q), self._p(saved["b5"]), self._p(fw.w_head), self._p(action), self._p(reward), B, A, 2 * h2, 2 * w2,
+                                             self._p(loss_terms), self._p(qsel), self._p(d_b5), self._p(dWp), self._p(dbp), self._p(dW_head), self._p(self.g["1.C1.bias"]),
+                                             self._st()), "gq_loss_head_bwd")
+        else:
+            weight = weight.to(self.dev, t.float32).reshape(B).contiguous()
+            self._ck(self.L.gq_loss_head_bwd_weighted(self._p(q), self._p(saved["b5"]), self._p(fw.w_head), self._p(action), self._p(reward), self._p(weight), B, A,
+                                                      2 * h2, 2 * w2, self._p(loss_terms), self._p(qsel), self._p(d_b5), self._p(dWp), self._p(dbp), self._p(dW_head),
+                                                      self._p(self.g["1.C1.bias"]), self._st()), "gq_loss_head_bwd_weighted")
         self.g["1.C1.weight"].copy_(dW_head.view(A, 64, 1, 1))
         ready("1.C1.")
         sv = saved["blocks"]
@@ -396,10 +408,12 @@ class QNetLearner:
         return loss_terms.mean(), qsel
 
     # ------------------------------------------------------------------ one learn() call
-    def learn_step(self, state, action, reward, return_pred=False):
+    def learn_step(self, state, action, reward, return_pred=False, weight=None):
         """state [B,4,H,W] f32 (what the agent stores in its replay buffer), action [B] or [B,1] flat indices rot*H*W + y*W + x, reward [B] or
         [B,1].  Returns the loss as a float (one device->host read, like the reference's `loss.item()`); with return_pred=True
-        (loss, q_pred [B] on the device), q_pred being the gathered Q-values of the training forward (Offline RL/train.py:109,122)."""
+        (loss, q_pred [B] on the device), q_pred being the gathered Q-values of the training forward (Offline RL/train.py:109,122).
+        weight: None (the reference's loss) or [B] f32 importance weights on the device; the step then minimises and returns the
+        weighted loss binary_cross_entropy(q_pred, reward, weight=weight)."""
         t = self.torch
         q, saved = self.forward_train(state)
         works = []
@@ -414,7 +428,7 @@ class QNetLearner:
             def on_ready(prefix):
                 works.append(dist.all_reduce(self.grad_slice(prefix), op=dist.ReduceOp.AVG, group=self.pg, async_op=True))
 
-        loss, qsel = self.backward(q, saved, action, reward, on_ready)
+        loss, qsel = self.backward(q, saved, action, reward, on_ready, weight)
         for w in works:
             w.wait()  # (stream-level wait: Adam below is ordered after the last piece)
         self.step_count += 1

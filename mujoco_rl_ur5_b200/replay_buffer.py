@@ -13,6 +13,7 @@ elements the reference's list sampling returns.  By default the generator is Pyt
 20 exactly like the reference (the unchanged agent draws its epsilon from the same stream); pass `rng=random.Random(20)` for
 a private stream (a generator passed in is used as it is, never re-seeded).  DeviceReplayBuffer's storage and gathers are tensor plumbing
 (any torch device); ObservationReplay, the online trainer's memory, stores observations and regenerates states with a kernel.
+PrioritizedObservationReplay replaces the uniform draw with prioritized replay (Schaul et al. 2016) on a device sum-tree.
 """
 import random as _random
 
@@ -131,3 +132,75 @@ class ObservationReplay(_Ring):
         states = fwd.obs_to_state_keyed(self.rgb, self.depth, self.envs.index_select(0, idx), self.steps.index_select(0, idx), seed, slot=idx,
                                         depth_threshold=depth_threshold, noise_std=noise_std)
         return states, self.actions.index_select(0, idx)[:, None], self.rewards.index_select(0, idx)[:, None]
+
+
+class PrioritizedObservationReplay(ObservationReplay):
+    """ObservationReplay with proportional prioritized replay (Schaul et al. 2016), on the GPU only (csrc/qnet_replay.cuh).  Slot i is
+    drawn with probability p_i / sum p, p_i = (|r - q_pred| + eps)^alpha from the last update that trained on it; a new transition
+    enters with the largest priority assigned so far (1.0 at the start).  `tree` [2 cap] f64 is the sum-tree over the slots
+    (cap = the smallest power of two >= size) and `pmax` [1] f64 that largest priority; both stay on the device.  The draw is
+    stratified (one uniform per 1/B of the total) and keyed on (seed, learner update, rank), so it needs no host generator and no
+    host-to-device copy.  Priorities are not part of a checkpoint, like the stored transitions themselves."""
+
+    def __init__(self, size, image_hw=(200, 200), device="cuda", alpha=0.6, eps=1e-6):
+        super().__init__(size, image_hw, device, rng=None, seed=None)  # the uniform generator is not used (and the global one not re-seeded)
+        from .qnet import load_qnet_library
+        from .qnet_learn import _bind_learn
+
+        t = self.torch
+        if self.device.type != "cuda":
+            raise RuntimeError("PrioritizedObservationReplay needs a CUDA device (there is no CPU fallback)")
+        self.L = _bind_learn(load_qnet_library())
+        self.alpha, self.eps = float(alpha), float(eps)
+        self.cap = 1 << max(0, (self.size - 1).bit_length())
+        self.tree = t.zeros(2 * self.cap, dtype=t.float64, device=self.device)
+        self.pmax = t.ones(1, dtype=t.float64, device=self.device)
+        self._claimed = None
+
+    def _ck(self, r, what):
+        if r != 0:
+            raise RuntimeError(f"{what} failed ({r}): {self.L.gq_last_error().decode()}")
+
+    def _st(self):
+        return self.torch.cuda.current_stream(self.device).cuda_stream
+
+    def _claim(self, n):
+        skip, idx = super()._claim(n)
+        self._claimed = idx
+        return skip, idx
+
+    def push_batch(self, rgb, depth, actions, rewards, envs, steps):
+        """ObservationReplay.push_batch, then the claimed slots' priorities := pmax (gq_per_push)"""
+        super().push_batch(rgb, depth, actions, rewards, envs, steps)
+        slots = self._claimed.contiguous()
+        self._ck(self.L.gq_per_push(self.tree.data_ptr(), self.pmax.data_ptr(), slots.data_ptr(), int(slots.numel()), self.cap, self._st()), "gq_per_push")
+
+    def sample_slots(self, batch_size, beta, seed, update, rank=0):
+        """-> (idx [B] int64, importance weights [B] f32), both on the device (gq_per_sample)"""
+        t = self.torch
+        if self.length == 0:
+            raise ValueError("sample from an empty replay")
+        idx = t.empty(batch_size, dtype=t.int64, device=self.device)
+        w = t.empty(batch_size, dtype=t.float32, device=self.device)
+        self._ck(self.L.gq_per_sample(self.tree.data_ptr(), self.cap, self.length, int(batch_size), float(beta), int(seed) & (2 ** 64 - 1),
+                                      int(update) & (2 ** 64 - 1), int(rank) & 0xFFFFFFFF, idx.data_ptr(), w.data_ptr(), self._st()), "gq_per_sample")
+        return idx, w
+
+    def sample(self, batch_size, fwd, seed, beta, update, rank=0, depth_threshold=1.1, noise_std=0.001):
+        """-> (states [B,4,H,W] f32, actions [B,1] int64, rewards [B,1] f32, idx [B] int64, weights [B] f32); the draw is keyed on
+        (seed, update, rank) - the trainer passes the learner's update count and its process rank - and the states are regenerated
+        by `fwd` (a QNetForward on this buffer's device) with the keyed transform under `seed`"""
+        idx, w = self.sample_slots(batch_size, beta, seed, update, rank)
+        states = fwd.obs_to_state_keyed(self.rgb, self.depth, self.envs.index_select(0, idx), self.steps.index_select(0, idx), seed, slot=idx,
+                                        depth_threshold=depth_threshold, noise_std=noise_std)
+        return states, self.actions.index_select(0, idx)[:, None], self.rewards.index_select(0, idx)[:, None], idx, w
+
+    def update_priorities(self, idx, qsel, reward):
+        """priorities of the slots idx [B] after training on them: (|reward - qsel| + eps)^alpha, in batch order (gq_per_update)"""
+        t = self.torch
+        idx = idx.to(self.device, t.int64).reshape(-1).contiguous()
+        B = int(idx.numel())
+        qsel = qsel.to(self.device, t.float32).reshape(B).contiguous()
+        reward = t.as_tensor(reward).to(self.device, t.float32).reshape(B).contiguous()
+        self._ck(self.L.gq_per_update(self.tree.data_ptr(), self.pmax.data_ptr(), idx.data_ptr(), qsel.data_ptr(), reward.data_ptr(), B, self.alpha,
+                                      self.eps, self.cap, self._st()), "gq_per_update")

@@ -49,8 +49,8 @@ int ge_destroy(ge_handle h);
  * there), 12 environments of the sub-step kernel resident per SM as granted by the occupancy API, 13 Hessian builds that used the
  * overflow row since ge_create (synchronises the engine's stream; saturates at INT_MAX).  Both builds read GE_HCAP at ge_create (hcap,
  * CTA-per-env build: from Σ tree blocks + 6 maxcon + 64 up to hfull; warp-per-env build: from the larger of Σ tree blocks and
- * 6 maxcon + 6 nbody up to hfull); the CTA-per-env build also reads GE_MAXCON (contact capacity, 16..512).  A value outside its range
- * is ignored, so size 6 / 10 tell what was used. */
+ * 6 maxcon + 6 nbody up to hfull); both also read GE_MAXCON (contact capacity, 16..512; the default hcap and the smallest GE_HCAP
+ * follow it).  A value outside its range is ignored, so size 6 / 10 tell what was used. */
 int ge_size(ge_handle h, int what);
 
 /* MujocoEnv.set_state + controller re-sync, as GraspEnv.reset_model does (GraspingEnv.py:466-470):

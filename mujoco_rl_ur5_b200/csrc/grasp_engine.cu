@@ -508,8 +508,10 @@ static void make_layout(const DevModel& m, Layout& L, const int* tree_dofnum_h, 
   L.sr = takeB(6 * GE_MAXSR);
   L.Ma = takeB(nv); L.grad = takeB(nv); L.search = takeB(nv); L.Mv = takeB(nv);
   L.Vb = takeB(6 * nb);
-  L.H = takeB(L.hcap);
-  L.Wb = L.hcap >= 6 * L.maxcon + 6 * nb ? L.H + 6 * L.maxcon : takeB(6 * nb);
+  // the region also holds the 6 maxcon contact wrenches, which a large contact capacity (GE_MAXCON) can make exceed the full triangle
+  const int hreg = L.hcap > 6 * L.maxcon ? L.hcap : 6 * L.maxcon;
+  L.H = takeB(hreg);
+  L.Wb = hreg >= 6 * L.maxcon + 6 * nb ? L.H + 6 * L.maxcon : takeB(6 * nb);
   end = endG;
   for (int e : {endT, endF, b}) if (e > end) end = e;
   L.fk_bytes = align_up(endG > endF ? endG : endF, 2) * 8;
@@ -650,7 +652,8 @@ extern "C" int ge_create(const void* model_blob, size_t nbytes, int n_envs, int 
   // overflow row in HBM.  The region must hold nt_update's contact and body wrenches, and the blocks of the mass solve (<= the tree
   // diagonal).
   {
-    const int maxcon = maxcon_default;
+    int maxcon = maxcon_default;
+    if (const char* ev = getenv("GE_MAXCON")) { int v = atoi(ev); if (v >= 16 && v <= 512) maxcon = v; }
     int need_min = 6 * maxcon + 6 * m.nbody;
     if (diag > need_min) need_min = diag;
     int cap = fit(maxcon, (233472 - 2 * (1024 + (long)run_attr.sharedSizeBytes)) / 10);

@@ -38,7 +38,9 @@ const char* ge_version(void);
 
 /* mujoco_py.load_model_from_path + MjSim (MujocoController.py:33-36) + MJ_Controller.create_lists (:136-254):
  * model_blob = compiled scene (mujoco_rl_ur5_b200/model/blob.py), copied to the device; n_envs independent copies of the
- * scene are created at qpos0 with the reference PID gains.  stream: cudaStream_t cast to void* (NULL = default). */
+ * scene are created at qpos0 with the reference PID gains.  stream: cudaStream_t cast to void* (NULL = default).
+ * GE_ERR_MODEL for a scene with more than 256 geoms (the renderer's per-tile geom list).  Engines of one scene with different
+ * workspace sizes (e.g. GE_MAXCON) may live side by side. */
 int ge_create(const void* model_blob /*[host]*/, size_t nbytes, int n_envs, int device, void* stream, ge_handle* out);
 int ge_destroy(ge_handle h);
 
@@ -111,11 +113,13 @@ int ge_step_open_loop(ge_handle h, int substeps, const uint8_t* env_mask);
 
 /* MJ_Controller.ik (MujocoController.py:467-517): xyz [N,3] -> q5 [N,5], ok [N] u8 (all [dev]) */
 int ge_ik(ge_handle h, const double* xyz, double* q5, uint8_t* ok);
-/* MJ_Controller.pixel_2_world (MujocoController.py:783-806): pixel_x, pixel_y [N] int32, depth [N] f32 -> xyz [N,3] f64 */
+/* MJ_Controller.pixel_2_world (MujocoController.py:783-806): pixel_x, pixel_y [N] int32, depth [N] f32 -> xyz [N,3] f64;
+ * GE_ERR_ARG for a camera outside [0, ncam) */
 int ge_pixel_2_world(ge_handle h, int cam, int width, int height, const int32_t* px, const int32_t* py, const float* depth, double* xyz);
 
 /* MJ_Controller.get_image_data + depth_2_meters (MujocoController.py:708-740): rgb [N,H,W,3] u8, depth_m [N,H,W] f32 [dev],
- * already flipped U/D + L/R like the reference; depth in metres */
+ * already flipped U/D + L/R like the reference; depth in metres.  GE_ERR_ARG for a camera outside [0, ncam) and for width or height
+ * outside [1, 32767] (the screen-space boxes of the geoms are 16-bit). */
 int ge_render(ge_handle h, int cam, int width, int height, uint8_t* rgb, float* depth_m);
 
 /* diagnostics for parity tests: copies one internal per-env field of env `env` to a host buffer after running the

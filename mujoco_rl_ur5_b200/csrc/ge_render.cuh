@@ -163,11 +163,12 @@ __device__ __forceinline__ double ray_geom(int g, const double* fr, const double
 }
 
 #define RTILE 16
+#define RTILE_LIST 256  // geoms a tile can list (ge_create rejects scenes with more)
 __global__ void __launch_bounds__(RTILE * RTILE) k_render(const double* gframes, const short4* gbox, const double* fpx, int n_env, int cam, int W, int H, unsigned char* rgb,
                                                           float* depth) {
   const DevModel& m = c_m;
-  __shared__ int s_list[256];
-  __shared__ short4 s_bb[256];  // screen-space box (pixel columns x..z, rows y..w) of the listed geom
+  __shared__ int s_list[RTILE_LIST];
+  __shared__ short4 s_bb[RTILE_LIST];  // screen-space box (pixel columns x..z, rows y..w) of the listed geom
   __shared__ int s_n;
   int env = blockIdx.y, tiles_x = (W + RTILE - 1) / RTILE;
   int tx = blockIdx.x % tiles_x, ty = blockIdx.x / tiles_x;
@@ -188,14 +189,14 @@ __global__ void __launch_bounds__(RTILE * RTILE) k_render(const double* gframes,
       const short4 bb = gb[g];
       if (bb.z < c0i || bb.x > c1i - 1 || bb.w < r0i || bb.y > r1i - 1) continue;
       int k = atomicAdd(&s_n, 1);
-      if (k < 256) { s_list[k] = g; s_bb[k] = bb; }
+      if (k < RTILE_LIST) { s_list[k] = g; s_bb[k] = bb; }
     }
   }
   __syncthreads();
   const double f = *fpx;
   int c = tx * RTILE + threadIdx.x, r = ty * RTILE + threadIdx.y;
   if (c >= W || r >= H) return;
-  int n = s_n < 256 ? s_n : 256;
+  int n = s_n < RTILE_LIST ? s_n : RTILE_LIST;
   double dc[3] = {(0.5 * W - c - 0.5) / f, (0.5 * H - r - 0.5) / f, -1.0}, dir[3];
   m3mulv(dir, cm, dc);
   double best = 1e300, bn[3] = {0, 0, 1};
@@ -238,8 +239,6 @@ static inline int render_launch(RenderCtx& rc, const DevModel& m, const Layout& 
     if (!rc.fpx && cudaMalloc(&rc.fpx, sizeof(double)) != cudaSuccess) return -1;
     rc.cap_envs = n_env;
   }
-  static bool attr_done = false;
-  if (!attr_done && L.fk_bytes > 48 * 1024) { cudaFuncSetAttribute(k_render_fk, cudaFuncAttributeMaxDynamicSharedMemorySize, L.fk_bytes); attr_done = true; }
   k_render_fk<<<n_env, GE_LANES, L.fk_bytes, stream>>>(qpos, n_env, rc.gframes, rc.gbox, rc.fpx, cam, W, H);
   int tiles = ((W + RTILE - 1) / RTILE) * ((H + RTILE - 1) / RTILE);
   dim3 grid(tiles, n_env), blk(RTILE, RTILE);

@@ -421,6 +421,7 @@ struct BlobEntry { char name[32]; int32_t dtype, ndim; int64_t shape[4]; int64_t
 
 struct ge_engine {
   int device, n_envs;
+  int ncam;          // cameras of the scene (ge_render / ge_pixel_2_world index cam_pos0 etc. with cam < ncam)
   cudaStream_t stream;
   DevModel hm;       // host copy of the struct holding DEVICE pointers
   Layout lay;
@@ -586,7 +587,7 @@ extern "C" int ge_create(const void* model_blob, size_t nbytes, int n_envs, int 
   auto PD = [&](const char* n) -> const double* { int64_t o = blob_off(B, n); if (o < 0) { missing = true; fail(GE_ERR_MODEL, "blob entry missing: %s", n); return nullptr; } return (const double*)((char*)h->dblob + o); };
   auto PI = [&](const char* n) -> const int* { int64_t o = blob_off(B, n); if (o < 0) { missing = true; fail(GE_ERR_MODEL, "blob entry missing: %s", n); return nullptr; } return (const int*)((char*)h->dblob + o); };
   m.nbody = I("nbody"); m.njnt = I("njnt"); m.nq = I("nq"); m.nv = I("nv"); m.nu = I("nu"); m.ngeom = I("ngeom"); m.neq = I("neq");
-  m.npair = I("npair"); m.nmesh = I("nmesh"); m.nM = I("nM"); m.ntree = I("ntree");
+  m.npair = I("npair"); m.nmesh = I("nmesh"); m.nM = I("nM"); m.ntree = I("ntree"); h->ncam = I("ncam");
   m.timestep = D("opt_timestep"); m.tolerance = D("opt_tolerance"); m.impratio = D("opt_impratio"); m.mpr_tol = D("opt_mpr_tolerance");
   m.meaninertia = D("stat_meaninertia"); m.extent = D("stat_extent"); m.zfar = D("vis_zfar");
   m.iterations = I("opt_iterations"); m.mpr_iter = I("opt_mpr_iterations"); m.ik_base_body = I("ik_base_body"); m.ee_body = I("ee_body");
@@ -615,6 +616,7 @@ extern "C" int ge_create(const void* model_blob, size_t nbytes, int n_envs, int 
   if (missing) { cudaFree(h->dblob); delete h; return GE_ERR_MODEL; }
   if (m.nu != GE_NU) { cudaFree(h->dblob); delete h; return fail(GE_ERR_MODEL, "model must have 7 actuators"); }
   if (m.ntree > 64) { cudaFree(h->dblob); delete h; return fail(GE_ERR_MODEL, "model has more than 64 kinematic trees"); }
+  if (m.ngeom > RTILE_LIST) { cudaFree(h->dblob); delete h; return fail(GE_ERR_MODEL, "model has more than 256 geoms (the renderer's tile list)"); }
   {
     int64_t cnt = 0;
     const int32_t* cd = (const int32_t*)blob_find(B, "pair_condim", &cnt);
@@ -722,11 +724,13 @@ extern "C" int ge_create(const void* model_blob, size_t nbytes, int n_envs, int 
   if (getenv("GE_VERBOSE"))
     fprintf(stderr, "grasp_engine: %s build, workspace %d B per env (%d doubles + %d ints), contacts <= %d, Hessian region %d of %d doubles, %d env(s) per CTA\n",
             GE_NW > 1 ? "CTA-per-env" : "warp-per-env", h->lay.total_bytes, h->lay.total_doubles, h->lay.total_ints, h->lay.maxcon, h->lay.hcap, h->lay.hfull, h->wpb);
-  if (h->ws_smem && h->lay.total_bytes > 48 * 1024) {
-    CK(cudaFuncSetAttribute(k_debug, cudaFuncAttributeMaxDynamicSharedMemorySize, h->lay.total_bytes));
-    CK(cudaFuncSetAttribute(k_step_open, cudaFuncAttributeMaxDynamicSharedMemorySize, h->lay.total_bytes));
+  // The opt-in to more than 48 KB of dynamic shared memory belongs to the kernel, not to this engine: every engine of this build in the
+  // process shares it.  Set to one engine's workspace, it would make the launches of another engine with a larger one fail.
+  for (const void* k : {(const void*)k_debug, (const void*)k_step_open, (const void*)k_body_xpos, (const void*)k_render_fk}) {
+    cudaFuncAttributes a;
+    CK(cudaFuncGetAttributes(&a, k));
+    CK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024 - (int)a.sharedSizeBytes));
   }
-  if (h->lay.fk_bytes > 48 * 1024) CK(cudaFuncSetAttribute(k_body_xpos, cudaFuncAttributeMaxDynamicSharedMemorySize, h->lay.fk_bytes));
   EnvArrays& E = h->E;
   size_t N = n_envs;
 #define AL(ptr, type, cnt) CK(cudaMalloc(&ptr, sizeof(type) * (cnt))); CK(cudaMemset(ptr, 0, sizeof(type) * (cnt)))
@@ -990,6 +994,7 @@ extern "C" int ge_ik(ge_handle h, const double* xyz, double* q5, uint8_t* ok) {
 }
 extern "C" int ge_pixel_2_world(ge_handle h, int cam, int width, int height, const int32_t* px, const int32_t* py, const float* depth, double* xyz) {
   if (!h || !px || !py || !depth || !xyz) return GE_ERR_ARG;
+  if (cam < 0 || cam >= h->ncam) return fail(GE_ERR_ARG, "ge_pixel_2_world: no such camera");
   if (bind(h)) return GE_ERR_CUDA;
   k_pixel_2_world<<<(h->n_envs + 127) / 128, 128, 0, h->stream>>>(h->n_envs, cam, width, height, px, py, depth, xyz);
   h->launches++;
@@ -998,6 +1003,8 @@ extern "C" int ge_pixel_2_world(ge_handle h, int cam, int width, int height, con
 }
 extern "C" int ge_render(ge_handle h, int cam, int width, int height, uint8_t* rgb, float* depth_m) {
   if (!h || !rgb || !depth_m || width <= 0 || height <= 0) return fail(GE_ERR_ARG, "ge_render: bad argument");
+  if (cam < 0 || cam >= h->ncam) return fail(GE_ERR_ARG, "ge_render: no such camera");
+  if (width > 32767 || height > 32767) return fail(GE_ERR_ARG, "ge_render: image width or height above 32767 (screen boxes are 16-bit)");
   if (bind(h)) return GE_ERR_CUDA;
   int r = render_launch(h->rctx, h->hm, h->lay, h->E.qpos, h->n_envs, cam, width, height, rgb, depth_m, h->stream, &h->launches);
   if (r) return fail(GE_ERR_CUDA, "ge_render: %s", cudaGetErrorString(cudaGetLastError()));

@@ -1601,6 +1601,84 @@ void orc_render(Env* e, int cam, int W, int H, uint8_t* rgb, float* depth) {
   }
 }
 
+/* ------------------------------------------------------------------ render probe: where rounding may decide a pixel.
+ * The CUDA renderer evaluates the same fp64 expressions as orc_render, but with FMA contraction and on geom frames from its own
+ * kinematics (which agree with fk's to rounding), so its f32 depth and u8 rgb can legitimately differ only where a rounding-sized
+ * change of the ray or of the frames changes the answer.  For each listed pixel (index r * W + c) this returns the geom orc_render
+ * picks (-1: background) and a bit set of such reasons:
+ *   1  the winner, its normal (by more than 1e-6), its f32 depth or its rgb changes when the ray direction moves by +-eps_px pixels
+ *      in x or y, or the camera origin by +-eps_m along a world axis (silhouettes, hull edges, frame differences);
+ *   2  the nearest hit of another geom is within a relative PROBE_REL_TIE of the winner's (coplanar faces);
+ *   4  a shaded channel base * shade * 255 + 0.5 lies within a relative 1e-9 of an integer (u8 truncation boundary);
+ *   8  the fp64 depth lies within a relative PROBE_REL_F32 of a rounding midpoint of f32;
+ *   16 a floor hit lies within 1e-9 m of a checker line (floor(hit / 0.25)). */
+#define PROBE_REL_TIE 1e-9
+#define PROBE_REL_F32 1e-12
+typedef struct { int g; double t, second, n[3]; float depth; uint8_t rgb[3]; double v[3]; double hit[3]; } ProbeHit;
+static void probe_trace(const Env* e, const double* o, const double* dir, ProbeHit* h) {
+  const Model* m = e->m;
+  h->g = -1; h->t = 1e300; h->second = 1e300; v3set(h->n, 0, 0, 1);
+  for (int g = 0; g < m->ngeom; g++) {
+    double n[3], t = ray_geom(e, g, o, dir, n);
+    if (!(t > 0)) continue;
+    if (t < h->t) { h->second = h->t; h->t = t; h->g = g; v3copy(h->n, n); }
+    else if (t < h->second) h->second = t;
+  }
+  if (h->g < 0) { h->depth = (float)(m->zfar * m->extent); h->rgb[0] = h->rgb[1] = h->rgb[2] = 0; return; }
+  h->depth = (float)h->t;
+  double light[3] = {-1, 1, -2.565};
+  v3normalize(light);
+  double lam = -v3dot(h->n, light);
+  if (lam < 0) lam = 0;
+  double shade = 0.4 + 0.6 * lam;
+  const double* col = m->geom_rgba + 4 * h->g;
+  double base[3] = {col[0], col[1], col[2]};
+  v3addscl(h->hit, o, dir, h->t);
+  if (m->geom_type[h->g] == G_PLANE) {
+    int cx = (int)floor(h->hit[0] / 0.25), cy = (int)floor(h->hit[1] / 0.25);
+    if ((cx + cy) & 1) { base[0] = 0.1; base[1] = 0.2; base[2] = 0.3; } else { base[0] = 0.2; base[1] = 0.3; base[2] = 0.4; }
+  }
+  for (int k = 0; k < 3; k++) { h->v[k] = base[k] * shade * 255.0 + 0.5; h->rgb[k] = (uint8_t)(h->v[k] > 255 ? 255 : h->v[k]); }
+}
+void orc_render_probe(Env* e, int cam, int W, int H, int n, const int64_t* pix, double eps_px, double eps_m, int* gid, int* flags) {
+  const Model* m = e->m;
+  fk(e);
+  const double *cp = m->cam_pos0 + 3 * cam, *cm = m->cam_mat0 + 9 * cam;
+  double f = 0.5 * H / tan(m->cam_fovy[cam] * M_PI / 360.0);
+  for (int i = 0; i < n; i++) {
+    int r = (int)(pix[i] / W), c = (int)(pix[i] % W), fl = 0;
+    double dc[3] = {(0.5 * W - c - 0.5) / f, (0.5 * H - r - 0.5) / f, -1.0}, dir[3];
+    m3mulv(dir, cm, dc);
+    ProbeHit h;
+    probe_trace(e, cp, dir, &h);
+    gid[i] = h.g;
+    if (h.g >= 0) {
+      if (h.second - h.t <= PROBE_REL_TIE * h.t) fl |= 2;
+      for (int k = 0; k < 3; k++) if (fabs(h.v[k] - floor(h.v[k] + 0.5)) <= 1e-9 * h.v[k]) fl |= 4;
+      float lo = nextafterf(h.depth, -INFINITY), hi = nextafterf(h.depth, INFINITY);
+      double mlo = 0.5 * ((double)h.depth + lo), mhi = 0.5 * ((double)h.depth + hi);
+      if (fabs(h.t - mlo) <= PROBE_REL_F32 * h.t || fabs(h.t - mhi) <= PROBE_REL_F32 * h.t) fl |= 8;
+      if (m->geom_type[h.g] == G_PLANE)
+        for (int k = 0; k < 2; k++) if (fabs(h.hit[k] - 0.25 * floor(h.hit[k] / 0.25 + 0.5)) <= 1e-9) fl |= 16;
+    }
+    for (int p = 0; p < 10; p++) {
+      double o2[3] = {cp[0], cp[1], cp[2]}, dc2[3] = {dc[0], dc[1], dc[2]}, dir2[3], s = (p & 1) ? -1.0 : 1.0;
+      if (p < 4) dc2[p >> 1] = (0.5 * (p < 2 ? W : H) - (p < 2 ? c : r) - 0.5 + s * eps_px) / f;
+      else o2[(p - 4) >> 1] += s * eps_m;
+      m3mulv(dir2, cm, dc2);
+      ProbeHit q;
+      probe_trace(e, o2, dir2, &q);
+      int moved = q.g != h.g;
+      if (!moved && h.g >= 0) {
+        for (int k = 0; k < 3; k++) moved |= fabs(q.n[k] - h.n[k]) > 1e-6 || q.rgb[k] != h.rgb[k];
+        moved |= q.depth != h.depth;
+      }
+      if (moved) { fl |= 1; break; }
+    }
+    flags[i] = fl;
+  }
+}
+
 /* ------------------------------------------------------------------ accessors for tests */
 double* orc_qpos(Env* e) { return e->qpos; }
 double* orc_qvel(Env* e) { return e->qvel; }

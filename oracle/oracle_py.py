@@ -61,6 +61,7 @@ def lib():
         L.orc_depth_2_meters.restype = C.c_double
         L.orc_depth_2_meters.argtypes = [P, C.c_double]
         L.orc_render.argtypes = [P, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_uint8), C.POINTER(C.c_float)]
+        L.orc_render_probe.argtypes = [P, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int64), C.c_double, C.c_double, I, I]
         L.orc_newton_stats.argtypes = [C.POINTER(C.c_long), C.c_int]
         _LIB = L
     return _LIB
@@ -244,3 +245,19 @@ class OracleEnv:
         depth = np.zeros((H, W), np.float32)
         self.L.orc_render(self.env, cam, W, H, rgb.ctypes.data_as(C.POINTER(C.c_uint8)), depth.ctypes.data_as(C.POINTER(C.c_float)))
         return rgb, depth
+
+    # flag bits of render_probe
+    PROBE_MOVES, PROBE_TIE, PROBE_RGB_ROUNDING, PROBE_F32_ROUNDING, PROBE_CHECKER = 1, 2, 4, 8, 16
+
+    def render_probe(self, cam, W, H, pixels=None, eps_px=1e-10, eps_m=1e-13):
+        """where rounding may decide a pixel of render(cam, W, H): for the flat pixel indices r * W + c (None: all), the geom render()
+        shows there (-1: background) and a bit set of reasons a renderer computing the same fp64 expressions with other rounding may
+        show something else (orc_render_probe in grasp_oracle.c).  Returns (gid, flags), int32 arrays shaped like `pixels`."""
+        pix = np.arange(W * H, dtype=np.int64) if pixels is None else np.ascontiguousarray(pixels, np.int64).ravel()
+        gid = np.zeros(len(pix), np.int32)
+        flags = np.zeros(len(pix), np.int32)
+        I = C.POINTER(C.c_int)
+        self.L.orc_render_probe(self.env, cam, W, H, len(pix), pix.ctypes.data_as(C.POINTER(C.c_int64)), float(eps_px), float(eps_m),
+                                gid.ctypes.data_as(I), flags.ctypes.data_as(I))
+        shape = (H, W) if pixels is None else np.shape(pixels)
+        return gid.reshape(shape), flags.reshape(shape)

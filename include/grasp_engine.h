@@ -29,8 +29,9 @@ enum { GE_OK = 0, GE_ERR_ARG = -1, GE_ERR_CUDA = -2, GE_ERR_MODEL = -3, GE_ERR_S
 enum { GE_MOVE_RUNNING = 0, GE_MOVE_SUCCESS = 1 /* "success" */, GE_MOVE_MAXSTEPS = 2 /* "max. steps reached: n" */,
        GE_MOVE_NO_IK = 3 /* "No valid joint angles received, could not move EE to position." */ };
 
-/* per-environment status bits (ge_get_status) */
-enum { GE_STATUS_CONTACT_OVERFLOW = 1, GE_STATUS_NONFINITE = 2, GE_STATUS_SOLVER_MAXITER = 4 };
+/* per-environment status bits (ge_get_status); ROW_OVERFLOW: more equality + joint-limit rows than the 16 simple-row slots, the
+ * later limit rows were dropped.  Bits 8..15 are the GE_NANCHECK probes. */
+enum { GE_STATUS_CONTACT_OVERFLOW = 1, GE_STATUS_NONFINITE = 2, GE_STATUS_SOLVER_MAXITER = 4, GE_STATUS_ROW_OVERFLOW = 8 };
 
 const char* ge_last_error(void);
 /* library / build identification: returns e.g. "grasp_engine 0.1 sm_90a fp64" */

@@ -127,7 +127,7 @@ __device__ __noinline__ int stage_constraints(double* ws, int* wi, int lane, int
     }
     nsr += total;
   }
-  if (nsr > GE_MAXSR) { nsr = GE_MAXSR; *status |= 1; }
+  if (nsr > GE_MAXSR) { nsr = GE_MAXSR; *status |= 8; }  // GE_STATUS_ROW_OVERFLOW
   body_vel(ws, qvel, lane);
   contact_base(ws, wi, ncon, c_vel(), lane);
   gsync();

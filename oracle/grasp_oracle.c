@@ -103,6 +103,7 @@ typedef struct {
   double *qM, *qLD, *qH, *qfrc_bias, *qfrc_passive, *qfrc_actuator, *qfrc_smooth, *qacc_smooth, *qfrc_constraint, *qacc;
   /* contacts + constraints */
   int ncon, nefc, ne, nl, nefc_max, maxcon; /* maxcon: contacts kept (<= MAXCON, orc_set_maxcon), later ones set con_overflow */
+  int maxsr, sr_overflow;                    /* maxsr: equality + limit rows kept (orc_set_maxsr; default: all), later ones set sr_overflow */
   Contact con[MAXCON];
   double *efc_J, *efc_B, *efc_pos, *efc_margin, *efc_diag, *efc_R, *efc_aref, *efc_force, *efc_AR;
   int* efc_type;
@@ -192,6 +193,7 @@ Env* orc_env_create(Model* m) {
   e->qacc_smooth = DALLOC(nv); e->qfrc_constraint = DALLOC(nv); e->qacc = DALLOC(nv);
   e->nefc_max = m->neq + m->njnt + 10 * MAXCON;
   e->maxcon = MAXCON;
+  e->maxsr = e->nefc_max;
   e->efc_J = DALLOC((size_t)e->nefc_max * nv); e->efc_B = DALLOC((size_t)e->nefc_max * nv);
   e->efc_pos = DALLOC(e->nefc_max); e->efc_margin = DALLOC(e->nefc_max); e->efc_diag = DALLOC(e->nefc_max);
   e->efc_R = DALLOC(e->nefc_max); e->efc_aref = DALLOC(e->nefc_max); e->efc_force = DALLOC(e->nefc_max); e->efc_AR = DALLOC(e->nefc_max);
@@ -993,14 +995,18 @@ static void make_constraint(Env* e) {
     }
   }
   e->ne = e->nefc;
-  /* joint limits (hinge / slide) */
+  e->sr_overflow = 0;
+  /* joint limits (hinge / slide), in joint order with the lower side first; rows past maxsr are dropped */
   for (int j = 0; j < m->njnt; j++) {
     if (!m->jnt_limited[j]) continue;
     int qa = m->jnt_qposadr[j], d = m->jnt_dofadr[j];
     double q = e->qpos[qa], mg = m->jnt_margin[j];
     for (int side = 0; side < 2; side++) {
       double dist = side == 0 ? q - m->jnt_range[2 * j] : m->jnt_range[2 * j + 1] - q;
-      if (dist < mg) { double* J = add_row(e, 1, dist, mg, m->dof_invweight0[d]); J[d] = side == 0 ? 1 : -1; }
+      if (!(dist < mg)) continue;
+      if (e->nefc >= e->maxsr) { e->sr_overflow = 1; continue; }
+      double* J = add_row(e, 1, dist, mg, m->dof_invweight0[d]);
+      J[d] = side == 0 ? 1 : -1;
     }
   }
   e->nl = e->nefc - e->ne;
@@ -1048,6 +1054,7 @@ static void make_constraint(Env* e) {
       for (int side = 0; side < 2; side++) {
         double dist = side == 0 ? q - m->jnt_range[2 * j] : m->jnt_range[2 * j + 1] - q;
         if (!(dist < mg)) continue;
+        if (i >= e->ne + e->nl) break;
         double imp, K, B, vel = 0;
         impedance(m->jnt_solref + 2 * j, m->jnt_solimp + 5 * j, e->efc_pos[i], mg, &imp, &K, &B, m->timestep);
         for (int d = 0; d < nv; d++) vel += e->efc_J[(size_t)i * nv + d] * e->qvel[d];
@@ -1693,6 +1700,13 @@ void orc_set_solver(Env* e, int solver) { e->solver = solver; }
 /* contact capacity: the list keeps the first n contacts of its emission order (analytic pairs, then MPR pairs, both in pair order),
  * like the CUDA engine's list of `maxcon` contacts; clamped to [0, MAXCON] */
 void orc_set_maxcon(Env* e, int n) { e->maxcon = n < 0 ? 0 : (n > MAXCON ? MAXCON : n); }
+/* simple-row capacity: make_constraint keeps the equality rows and then the first limit rows (joint order, lower side first) up to
+ * n rows in all, like the CUDA engine's GE_MAXSR slots; n < 0 restores the default (no cap) */
+void orc_set_maxsr(Env* e, int n) { e->maxsr = n < 0 ? e->nefc_max : n; }
+/* 1 if the last make_constraint dropped limit rows at the simple-row capacity */
+int orc_sr_overflow(Env* e) { return e->sr_overflow; }
+/* rows of the last make_constraint: out[0] equality, out[1] joint limit, out[2] contact */
+void orc_efc_split(Env* e, int* out) { out[0] = e->ne; out[1] = e->nl; out[2] = e->nefc - e->ne - e->nl; }
 /* 1 if the last collision stage found more contacts than the capacity */
 int orc_con_overflow(Env* e) { return e->con_overflow; }
 /* broad-phase survivors of the last collision stage (the engine's "ncand") */

@@ -45,6 +45,9 @@ def lib():
         L.orc_set_solver.argtypes = [P, C.c_int]
         L.orc_set_maxcon.argtypes = [P, C.c_int]
         L.orc_con_overflow.argtypes = [P]
+        L.orc_set_maxsr.argtypes = [P, C.c_int]
+        L.orc_sr_overflow.argtypes = [P]
+        L.orc_efc_split.argtypes = [P, I]
         L.orc_ncand.argtypes = [P]
         L.orc_reset.argtypes = [P, D, D]
         L.orc_field.restype = D
@@ -151,6 +154,23 @@ class OracleEnv:
     def con_overflow(self):
         """1 if the last collision stage found more contacts than the capacity"""
         return int(self.L.orc_con_overflow(self.env))
+
+    def set_maxsr(self, n=-1):
+        """simple-row capacity: the equality rows and then the first limit rows (joint order, lower side first) up to n rows in all
+        are kept, later limit rows are dropped and `sr_overflow` is set, as in the CUDA engine's GE_MAXSR slots (n < 0: no cap)"""
+        self.L.orc_set_maxsr(self.env, int(n))
+
+    @property
+    def sr_overflow(self):
+        """1 if the last forward() dropped limit rows at the simple-row capacity"""
+        return int(self.L.orc_sr_overflow(self.env))
+
+    @property
+    def efc_split(self):
+        """constraint rows of the last forward(): (equality, joint limit, contact)"""
+        out = (C.c_int * 3)()
+        self.L.orc_efc_split(self.env, out)
+        return tuple(int(v) for v in out)
 
     @property
     def ncand(self):

@@ -50,12 +50,10 @@ int gq_bn_act(const float* x, const float* stats, const float* gamma, const floa
               float eps, void* stream);
 /* nn.UpsamplingBilinear2d(scale_factor=2) (align_corners=True) (Modules.py:248,250): x [B,H,W,C] -> y [B,2H,2W,C] */
 int gq_upsample2x(const void* x, void* y, int B, int H, int W, int C, void* stream);
-/* Grasping_Module_multidiscrete.C1 = nn.Conv2d(64, A, 1) + squeeze + Sigmoid (Modules.py:251,281-283): x [B,HW,64] bf16, w [A][64] f32,
- * bias [A] f32 -> q [B,A,HW] f32 (the reference's NCHW output layout) */
-int gq_head(const void* x, const float* w, const float* bias, float* q, int B, int HW, int A, void* stream);
-/* The same tail computed at the lower resolution: Grasping_Module_multidiscrete ends with UP2 -> C1 -> sigmoid (Modules.py:250-251,281-283) and
- * C1 (1x1 conv + bias) commutes with bilinear up-sampling, so q = sigmoid(UP2(C1(x))): x [B,H,W,64] bf16 (the input of UP2),
- * scratch_z [B,A,H,W] f32, q [B,A,2H,2W] f32 */
+/* Network tail computed at the lower resolution: Grasping_Module_multidiscrete ends with UP2 -> C1 = nn.Conv2d(64, A, 1) -> squeeze ->
+ * Sigmoid (Modules.py:250-251,281-283) and C1 (1x1 conv + bias) commutes with bilinear up-sampling, so q = sigmoid(UP2(C1(x))):
+ * x [B,H,W,64] bf16 (the input of UP2), w [A][64] f32, bias [A] f32 (A <= 8), scratch_z [B,A,H,W] f32, q [B,A,2H,2W] f32 (the
+ * reference's NCHW output layout) */
 int gq_head_up2(const void* x, const float* w, const float* bias, float* scratch_z, float* q, int B, int H, int W, int A, void* stream);
 /* Grasp_Agent.transform_observation(normalize=True, jitter_and_noise=False) batched (Grasping_Agent_multidiscrete.py:301-368):
  * rgb [B,HW,3] u8, depth [B,HW] f32 metres -> state [B,4,HW] f32 (rgb/255, depth clipped at depth_threshold, negated, min-max per image);
@@ -120,7 +118,7 @@ int gq_loss_head_bwd_weighted(const float* q, const void* x, const float* w_head
                               int A, int H, int W, float* loss_terms, float* qsel, void* dX, float* dW_partial, float* db_partial, float* dW_head,
                               float* db_head, void* stream);
 /* backward of y = relu(BatchNorm(o) [+ identity]) with batch statistics (BasicBlock, Modules.py:128-142): dY, act = y [B,HW,C] bf16, o [B,HW,C] f32,
- * stats merged [B,C,2], gamma [C].  Out: d_o [B,HW,C] bf16 (gradient w.r.t. the convolution output), dgamma, dbeta [C] (either may be NULL),
+ * stats merged [B,C,2], gamma [C], C a multiple of 8.  Out: d_o [B,HW,C] bf16 (gradient w.r.t. the convolution output), dgamma, dbeta [C] (either may be NULL),
  * dpre_out (NULL or [B,HW,C] bf16) = dY * (y > 0), the gradient that also enters the identity branch.
  * scratch_part: ceil(B*HW/128) * C * 2 floats, scratch_sums: 2 C floats. */
 int gq_bn_relu_bwd(const void* dY, const void* act, const float* o, const float* stats, const float* gamma, int B, int HW, int C, float eps,
@@ -131,7 +129,7 @@ int gq_conv_wgrad(const void* dY, const void* x, float* scratch_part, float* dW,
 /* weight gradient of Perception_Module.C1 (4 -> 64, Modules.py:163): dY [B,H,W,64] bf16, x [B,4,H,W] f32 -> dW [64][3][3][4] f32;
  * scratch_part: ceil(B*H*W/2048) * 64 * 36 floats */
 int gq_conv_first_wgrad(const void* dY, const float* x, float* scratch_part, float* dW, int B, int H, int W, void* stream);
-/* MaxPool2d(3, 2, 1) backward: x [B,H,W,C] bf16 (pool input), dY [B,ceil(H/2),ceil(W/2),C] bf16 -> dX [B,H,W,C] bf16 */
+/* MaxPool2d(3, 2, 1) backward: x [B,H,W,C] bf16 (pool input), dY [B,ceil(H/2),ceil(W/2),C] bf16 -> dX [B,H,W,C] bf16; C a multiple of 8 */
 int gq_maxpool_bwd(const void* x, const void* dY, void* dX, int B, int H, int W, int C, void* stream);
 /* UpsamplingBilinear2d(2) backward: dY [B,2H,2W,C] bf16 -> dX [B,H,W,C] bf16 */
 int gq_upsample2x_bwd(const void* dY, void* dX, int B, int H, int W, int C, void* stream);

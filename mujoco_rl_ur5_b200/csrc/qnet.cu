@@ -13,7 +13,6 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
-#include <stdlib.h>
 #include <string.h>
 
 #include "../../include/grasp_qnet.h"
@@ -258,42 +257,10 @@ __global__ void k_bn_reduce(const float* __restrict__ part, float* __restrict__ 
 }
 
 // ------------------------------------------------------------------------------------------------ small layers
-// first conv: x [B,4,H,W] f32 (NCHW, the agent's tensor), w [64][3][3][4] f32 -> y [B,H,W,64] bf16; no BN / ReLU follows (Modules.py:176)
-__global__ void k_conv_first(const float* __restrict__ x, const float* __restrict__ w, bf16* __restrict__ y, int B, int H, int W) {
-  __shared__ __align__(16) float sw[64 * 36];
-  for (int i = threadIdx.x; i < 64 * 36; i += blockDim.x) sw[i] = w[i];
-  __syncthreads();
-  int p = blockIdx.x * blockDim.x + threadIdx.x, HW = H * W;
-  if (p >= B * HW) return;
-  int b = p / HW, oh = (p % HW) / W, ow = p % W;
-  float in[36];
-#pragma unroll
-  for (int t = 0; t < 9; t++) {
-    int ih = oh + t / 3 - 1, iw = ow + t % 3 - 1;
-    bool ok = ih >= 0 && ih < H && iw >= 0 && iw < W;
-#pragma unroll
-    for (int c = 0; c < 4; c++) in[t * 4 + c] = ok ? x[((size_t)(b * 4 + c) * H + ih) * W + iw] : 0.f;
-  }
-  bf16* out = y + (size_t)p * 64;
-  const float4* sw4 = (const float4*)sw;  // 9 x 16-byte broadcast reads per output channel instead of 36 scalar ones
-  for (int co = 0; co < 64; co += 8) {
-    __nv_bfloat162 o[4];
-#pragma unroll
-    for (int h = 0; h < 4; h++) {
-      float a0 = 0, a1 = 0;
-#pragma unroll
-      for (int k = 0; k < 9; k++) {
-        float4 w0 = sw4[(co + 2 * h) * 9 + k], w1 = sw4[(co + 2 * h + 1) * 9 + k];
-        a0 += in[4 * k] * w0.x; a0 += in[4 * k + 1] * w0.y; a0 += in[4 * k + 2] * w0.z; a0 += in[4 * k + 3] * w0.w;
-        a1 += in[4 * k] * w1.x; a1 += in[4 * k + 1] * w1.y; a1 += in[4 * k + 2] * w1.z; a1 += in[4 * k + 3] * w1.w;
-      }
-      o[h] = __floats2bfloat162_rn(a0, a1);
-    }
-    *(uint4*)(out + co) = *(uint4*)o;
-  }
-}
-// same layer, two horizontally consecutive pixels per thread: every weight vector read from shared memory feeds both (half the LDS
-// traffic per FMA, the limiter of the one-pixel version); pixel pairs are taken along the flattened index, B*H*W must be even
+// first conv: x [B,4,H,W] f32 (NCHW, the agent's tensor), w [64][3][3][4] f32 -> y [B,H,W,64] bf16; no BN / ReLU follows (Modules.py:176).
+// Two consecutive pixels of the flattened index per thread: every weight vector read from shared memory feeds both (half the LDS
+// traffic per FMA of a kernel with one pixel per thread).  When B*H*W is odd, the last thread computes its one pixel twice and stores it once
+// (clamping its index keeps 126 registers = four CTAs per SM; selecting the pixel took 130 registers and left room for three).
 __global__ void __launch_bounds__(128) k_conv_first2(const float* __restrict__ x, const float* __restrict__ w, bf16* __restrict__ y, int B, int H, int W) {
   __shared__ __align__(16) float sw[64 * 36];
   for (int i = threadIdx.x; i < 64 * 36; i += blockDim.x) sw[i] = w[i];
@@ -304,7 +271,7 @@ __global__ void __launch_bounds__(128) k_conv_first2(const float* __restrict__ x
   float in[2][36];
 #pragma unroll
   for (int q = 0; q < 2; q++) {
-    const int p = p0 + q, b = p / HW, oh = (p % HW) / W, ow = p % W;
+    const int p = min(p0 + q, B * HW - 1), b = p / HW, oh = (p % HW) / W, ow = p % W;
 #pragma unroll
     for (int t = 0; t < 9; t++) {
       const int ih = oh + t / 3 - 1, iw = ow + t % 3 - 1;
@@ -324,7 +291,7 @@ __global__ void __launch_bounds__(128) k_conv_first2(const float* __restrict__ x
       for (int k = 0; k < 9; k++) {
         const float4 w0 = sw4[(co + 2 * h) * 9 + k], w1 = sw4[(co + 2 * h + 1) * 9 + k];
 #pragma unroll
-        for (int q = 0; q < 2; q++) {  // same accumulation order per output as k_conv_first
+        for (int q = 0; q < 2; q++) {  // every output: one chain over the taps and input channels in order, whatever the pixel count
           a[q][0] += in[q][4 * k] * w0.x; a[q][0] += in[q][4 * k + 1] * w0.y; a[q][0] += in[q][4 * k + 2] * w0.z; a[q][0] += in[q][4 * k + 3] * w0.w;
           a[q][1] += in[q][4 * k] * w1.x; a[q][1] += in[q][4 * k + 1] * w1.y; a[q][1] += in[q][4 * k + 2] * w1.z; a[q][1] += in[q][4 * k + 3] * w1.w;
         }
@@ -332,7 +299,7 @@ __global__ void __launch_bounds__(128) k_conv_first2(const float* __restrict__ x
       o[0][h] = __floats2bfloat162_rn(a[0][0], a[0][1]); o[1][h] = __floats2bfloat162_rn(a[1][0], a[1][1]);
     }
     *(uint4*)(out + co) = *(uint4*)o[0];
-    *(uint4*)(out + 64 + co) = *(uint4*)o[1];
+    if (p0 + 1 < B * HW) *(uint4*)(out + 64 + co) = *(uint4*)o[1];
   }
 }
 // MaxPool2d(kernel 3, stride 2, padding 1) on NHWC bf16
@@ -419,10 +386,9 @@ __global__ void k_upsample2x(const bf16* __restrict__ x, bf16* __restrict__ y, i
   }
   *(uint4*)(y + p * C + cv) = *(uint4*)o;
 }
-// last layer: conv1x1 64 -> A (+bias) and sigmoid; x [B,HW,64] bf16, w [A][64] f32 -> q [B,A,HW] f32 (NCHW like the reference output)
-// SIGMOID = false writes the pre-activation (used at low resolution by gq_head_up2)
-template <bool SIGMOID>
-__global__ void k_head(const bf16* __restrict__ x, const float* __restrict__ w, const float* __restrict__ bias, float* __restrict__ q, int B, int HW, int A) {
+// last layer: conv1x1 64 -> A (+bias) before the sigmoid; x [B,HW,64] bf16, w [A][64] f32 -> z [B,A,HW] f32 (NCHW like the reference
+// output).  gq_head_up2 runs it on the low-resolution map and k_up2_sigmoid finishes the layer.
+__global__ void k_head(const bf16* __restrict__ x, const float* __restrict__ w, const float* __restrict__ bias, float* __restrict__ z, int B, int HW, int A) {
   __shared__ __align__(16) float sw[8 * 64 + 8];
   for (int i = threadIdx.x; i < A * 64; i += blockDim.x) sw[i] = w[i];
   if (threadIdx.x < A) sw[8 * 64 + threadIdx.x] = bias[threadIdx.x];
@@ -446,7 +412,7 @@ __global__ void k_head(const bf16* __restrict__ x, const float* __restrict__ w, 
       float4 wv = ((const float4*)sw)[a * 16 + c];
       acc += in[4 * c] * wv.x; acc += in[4 * c + 1] * wv.y; acc += in[4 * c + 2] * wv.z; acc += in[4 * c + 3] * wv.w;
     }
-    q[((size_t)b * A + a) * HW + pix] = SIGMOID ? 1.f / (1.f + __expf(-acc)) : acc;
+    z[((size_t)b * A + a) * HW + pix] = acc;
   }
 }
 // q = sigmoid(UpsamplingBilinear2d(2)(z)) on A planes: z [B*A, H, W] f32 -> q [B*A, 2H, 2W] f32 (align_corners=True).
@@ -921,10 +887,7 @@ extern "C" int gq_conv_tc_fused(const void* a, const void* x, const void* w, con
   return 0;
 }
 extern "C" int gq_conv_first(const float* x, const float* w, void* y, int B, int H, int W, void* stream) {
-  static int one_pixel = -1;
-  if (one_pixel < 0) { const char* e = getenv("GQ_FIRST1"); one_pixel = (e && atoi(e) != 0) ? 1 : 0; }  // GQ_FIRST1=1: one pixel per thread
-  if (one_pixel || ((size_t)B * H * W) % 2) k_conv_first<<<(B * H * W + 127) / 128, 128, 0, (cudaStream_t)stream>>>(x, w, (bf16*)y, B, H, W);
-  else k_conv_first2<<<(B * H * W / 2 + 127) / 128, 128, 0, (cudaStream_t)stream>>>(x, w, (bf16*)y, B, H, W);
+  k_conv_first2<<<((B * H * W + 1) / 2 + 127) / 128, 128, 0, (cudaStream_t)stream>>>(x, w, (bf16*)y, B, H, W);
   QCK(cudaGetLastError());
   return 0;
 }
@@ -956,16 +919,10 @@ extern "C" int gq_upsample2x(const void* x, void* y, int B, int H, int W, int C,
   QCK(cudaGetLastError());
   return 0;
 }
-extern "C" int gq_head(const void* x, const float* w, const float* bias, float* q, int B, int HW, int A, void* stream) {
-  if (A > 8) { snprintf(q_err, sizeof q_err, "gq_head: at most 8 action channels"); return -1; }
-  k_head<true><<<(unsigned)(((size_t)B * HW + 127) / 128), 128, 0, (cudaStream_t)stream>>>((const bf16*)x, w, bias, q, B, HW, A);
-  QCK(cudaGetLastError());
-  return 0;
-}
 extern "C" int gq_head_up2(const void* x, const float* w, const float* bias, float* scratch_z, float* q, int B, int H, int W, int A, void* stream) {
   if (A > 8 || !scratch_z) { snprintf(q_err, sizeof q_err, "gq_head_up2: bad argument"); return -1; }
   cudaStream_t st = (cudaStream_t)stream;
-  k_head<false><<<(unsigned)(((size_t)B * H * W + 127) / 128), 128, 0, st>>>((const bf16*)x, w, bias, scratch_z, B, H * W, A);
+  k_head<<<(unsigned)(((size_t)B * H * W + 127) / 128), 128, 0, st>>>((const bf16*)x, w, bias, scratch_z, B, H * W, A);
   size_t n = (size_t)B * A * 4 * H * W;
   k_up2_sigmoid<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(scratch_z, q, B * A, H, W);
   QCK(cudaGetLastError());

@@ -13,8 +13,7 @@
 //   dgrad (gradient w.r.t. the convolution input) = the forward wgmma convolution applied to dY with the spatially flipped,
 //          in/out-transposed weights (gq_conv_tc called by the host wrapper);
 //   wgrad (gradient w.r.t. the weights)           = k_wgrad_wgmma below: wgmma GEMM with K = pixels, both operands MN-major straight from the
-//          NHWC tensors by TMA (k_wgrad, a CUDA-core tiled kernel, is its A/B partner), split-K over the images of the batch (partials
-//          reduced in image order: deterministic);
+//          NHWC tensors by TMA, split-K over the images of the batch (partials reduced in image order: deterministic);
 //   everything else is element-wise / reduction glue.
 // Included at the end of qnet.cu (same library, C-ABI in include/grasp_qnet.h).
 #pragma once
@@ -112,7 +111,7 @@ __global__ void k_reduce_rows(const float* __restrict__ part, float* __restrict_
 // dY [B*HW, C] bf16 gradient w.r.t. y, act [B*HW, C] bf16 = y (ReLU mask: y > 0), o [B*HW, C] fp32 pre-BN convolution output.
 // Pass 1 (k_bn_bwd_reduce): per CTA (a block of rows) and channel: sum dpre, sum dpre * xhat, with dpre = dY * (y > 0); optionally
 //         writes dpre as bf16 (the gradient that also flows into the shortcut convolution / the identity branch).
-// Pass 2 (k_bn_bwd_apply):  d_o = gamma * rstd * (dpre - S1 / N - xhat * S2 / N) as bf16;  dgamma = S2, dbeta = S1.
+// Pass 2 (k_bn_bwd_apply8): d_o = gamma * rstd * (dpre - S1 / N - xhat * S2 / N) as bf16;  dgamma = S2, dbeta = S1.
 __global__ void __launch_bounds__(256) k_bn_bwd_reduce(const bf16* __restrict__ dY, const bf16* __restrict__ act, const float* __restrict__ o,
                                                        const float* __restrict__ stats, int rows, int C, int HW, float eps, int rows_per_cta,
                                                        bf16* __restrict__ dpre_out, float* __restrict__ part) {
@@ -162,20 +161,7 @@ __global__ void __launch_bounds__(128) k_bn_bwd_sums(const float* __restrict__ p
     if (dbeta) dbeta[c] = (float)a1;
   }
 }
-__global__ void __launch_bounds__(256) k_bn_bwd_apply(const bf16* __restrict__ dY, const bf16* __restrict__ act, const float* __restrict__ o,
-                                                      const float* __restrict__ stats, const float* __restrict__ gamma, const float* __restrict__ sums,
-                                                      size_t n, int C, int HW, float invN, float eps, bf16* __restrict__ d_o) {
-  size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  const int c = (int)(i % C);
-  const float s1 = stats[(size_t)c * 2], s2 = stats[(size_t)c * 2 + 1];
-  const float mean = s1 / HW, var = fmaxf(s2 / HW - mean * mean, 0.f), rstd = rsqrtf(var + eps);
-  const float xhat = (o[i] - mean) * rstd;
-  const float d = __bfloat162float(act[i]) > 0.f ? __bfloat162float(dY[i]) : 0.f;
-  d_o[i] = __float2bfloat16(gamma[c] * rstd * (d - sums[c * 2] * invN - xhat * sums[c * 2 + 1] * invN));
-}
-
-// the same, 8 consecutive channels per thread (16-byte loads / stores; C % 8 == 0), identical arithmetic per element
+// pass 2, 8 consecutive channels per thread (16-byte loads / stores; C % 8 == 0)
 __global__ void __launch_bounds__(256) k_bn_bwd_apply8(const bf16* __restrict__ dY, const bf16* __restrict__ act, const float* __restrict__ o,
                                                        const float* __restrict__ stats, const float* __restrict__ gamma, const float* __restrict__ sums,
                                                        size_t n8, int C, int HW, float invN, float eps, bf16* __restrict__ d_o) {
@@ -204,77 +190,6 @@ __global__ void __launch_bounds__(256) k_bn_bwd_apply8(const bf16* __restrict__ 
     out[k] = __floats2bfloat162_rn(r[0], r[1]);
   }
   *(uint4*)(d_o + i) = *(const uint4*)out;
-}
-
-// ------------------------------------------------------------------------------------------------ weight gradient of a convolution
-// dW[co][tap][ci] = sum over images b and pixels p of dY[b,p,co] * X[b, p + tap, ci]  (zero outside the image).
-// grid (Cout / 64, Cin / 64, taps * B): one CTA = a 64 x 64 tile of (co, ci) for one tap and ONE image (split-K over the batch; the
-// partials [B][Cout][taps][Cin] are summed in image order by k_reduce_rows).  256 threads, each a 4 x 4 register tile; the K loop runs
-// over the pixels in chunks of 32 rows staged through shared memory (rows of dY / X are channel-contiguous: coalesced 128-byte reads).
-#define WG_T 64
-#define WG_K 32
-__global__ void __launch_bounds__(256) k_wgrad(const bf16* __restrict__ dY, const bf16* __restrict__ X, float* __restrict__ part, int H, int W, int Cin, int Cout,
-                                               int ks) {
-  __shared__ float sA[WG_K][WG_T + 4];  // dY chunk [pixel][co]
-  __shared__ float sB[WG_K][WG_T + 4];  // X chunk  [pixel][ci]
-  const int taps = ks * ks, pad = ks / 2;
-  const int co0 = blockIdx.x * WG_T, ci0 = blockIdx.y * WG_T, tap = blockIdx.z % taps, b = blockIdx.z / taps;
-  const int dh = tap / ks - pad, dw = tap % ks - pad, HW = H * W;
-  const int tid = threadIdx.x, tm = (tid / 16) * 4, tn = (tid % 16) * 4;  // 16 x 16 threads, 4 x 4 outputs each
-  float acc[4][4];
-#pragma unroll
-  for (int i = 0; i < 4; i++)
-#pragma unroll
-    for (int j = 0; j < 4; j++) acc[i][j] = 0.f;
-  const bf16* dYb = dY + (size_t)b * HW * Cout;
-  const bf16* Xb = X + (size_t)b * HW * Cin;
-  const int lr = tid / 8, lc = (tid % 8) * 8;  // loader: row lr of the chunk, 8 consecutive channels starting at lc
-  for (int p0 = 0; p0 < HW; p0 += WG_K) {
-    {
-      const int p = p0 + lr;
-      float va[8], vb[8];
-      const bool okp = p < HW;
-      const int oh = okp ? p / W : 0, ow = okp ? p - oh * W : 0, ih = oh + dh, iw = ow + dw;
-      const bool okx = okp && ih >= 0 && ih < H && iw >= 0 && iw < W;
-      if (okp) {
-        const uint4 qa = *(const uint4*)(dYb + (size_t)p * Cout + co0 + lc);
-        const __nv_bfloat162* pa = (const __nv_bfloat162*)&qa;
-#pragma unroll
-        for (int k = 0; k < 4; k++) { const float2 f = __bfloat1622float2(pa[k]); va[2 * k] = f.x; va[2 * k + 1] = f.y; }
-      } else {
-#pragma unroll
-        for (int k = 0; k < 8; k++) va[k] = 0.f;
-      }
-      if (okx) {
-        const uint4 qb = *(const uint4*)(Xb + ((size_t)ih * W + iw) * Cin + ci0 + lc);
-        const __nv_bfloat162* pb = (const __nv_bfloat162*)&qb;
-#pragma unroll
-        for (int k = 0; k < 4; k++) { const float2 f = __bfloat1622float2(pb[k]); vb[2 * k] = f.x; vb[2 * k + 1] = f.y; }
-      } else {
-#pragma unroll
-        for (int k = 0; k < 8; k++) vb[k] = 0.f;
-      }
-#pragma unroll
-      for (int k = 0; k < 8; k++) { sA[lr][lc + k] = va[k]; sB[lr][lc + k] = vb[k]; }
-    }
-    __syncthreads();
-#pragma unroll 8
-    for (int k = 0; k < WG_K; k++) {
-      float a[4], bb[4];
-#pragma unroll
-      for (int i = 0; i < 4; i++) { a[i] = sA[k][tm + i]; bb[i] = sB[k][tn + i]; }
-#pragma unroll
-      for (int i = 0; i < 4; i++)
-#pragma unroll
-        for (int j = 0; j < 4; j++) acc[i][j] += a[i] * bb[j];
-    }
-    __syncthreads();
-  }
-  float* out = part + (size_t)b * Cout * taps * Cin;
-#pragma unroll
-  for (int i = 0; i < 4; i++)
-#pragma unroll
-    for (int j = 0; j < 4; j++) out[((size_t)(co0 + tm + i) * taps + tap) * Cin + ci0 + tn + j] = acc[i][j];
 }
 
 // first convolution (4 -> 64 channels, 3x3, no bias; Modules.py:163): dW[co][tap][c] = sum_{b,p} dY[b,p,co] * x[b,c,p+tap] with x the
@@ -316,30 +231,8 @@ __global__ void __launch_bounds__(256) k_conv_first_wgrad(const bf16* __restrict
 
 // ------------------------------------------------------------------------------------------------ pooling / up-sampling backward, glue
 // MaxPool2d(3, stride 2, padding 1) backward in gather form: input pixel (ih, iw) receives dY of every window whose arg-max it is
-// (first maximum in window scan order, as PyTorch does).  x [B,H,W,C] bf16 (the pool's input), dY [B,OH,OW,C] bf16 -> dX [B,H,W,C] bf16
-__global__ void k_maxpool_bwd(const bf16* __restrict__ x, const bf16* __restrict__ dY, bf16* __restrict__ dX, int B, int H, int W, int C) {
-  const int OH = (H + 1) / 2, OW = (W + 1) / 2;
-  size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x, n = (size_t)B * H * W * C;
-  if (i >= n) return;
-  const int c = (int)(i % C), iw = (int)((i / C) % W), ih = (int)((i / ((size_t)C * W)) % H), b = (int)(i / ((size_t)C * W * H));
-  float g = 0.f;
-  // windows (oh, ow) that contain (ih, iw): oh*2-1 <= ih <= oh*2+1
-  for (int oh = (ih) / 2; oh <= (ih + 1) / 2 && oh < OH; oh++)
-    for (int ow = (iw) / 2; ow <= (iw + 1) / 2 && ow < OW; ow++) {
-      // arg-max of the window
-      float best = -3.0e38f; int bh = -1, bw = -1;
-      for (int kh = 0; kh < 3; kh++)
-        for (int kw = 0; kw < 3; kw++) {
-          const int hh = oh * 2 - 1 + kh, ww = ow * 2 - 1 + kw;
-          if (hh < 0 || hh >= H || ww < 0 || ww >= W) continue;
-          const float v = __bfloat162float(x[(((size_t)b * H + hh) * W + ww) * C + c]);
-          if (v > best) { best = v; bh = hh; bw = ww; }
-        }
-      if (bh == ih && bw == iw) g += __bfloat162float(dY[(((size_t)b * OH + oh) * OW + ow) * C + c]);
-    }
-  dX[i] = __float2bfloat16(g);
-}
-// the same, 8 channels per thread (16-byte loads; C % 8 == 0): identical arithmetic and window order, an eighth of the load instructions
+// (first maximum in window scan order, as PyTorch does).  x [B,H,W,C] bf16 (the pool's input), dY [B,OH,OW,C] bf16 -> dX [B,H,W,C] bf16;
+// 8 channels per thread (16-byte loads; C % 8 == 0)
 __global__ void __launch_bounds__(256) k_maxpool_bwd8(const bf16* __restrict__ x, const bf16* __restrict__ dY, bf16* __restrict__ dX, int B, int H, int W, int C) {
   const int OH = (H + 1) / 2, OW = (W + 1) / 2, C8 = C / 8;
   size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x, n = (size_t)B * H * W * C8;
@@ -485,23 +378,21 @@ extern "C" int gq_loss_head_bwd_weighted(const float* q, const void* x, const fl
 extern "C" int gq_bn_relu_bwd(const void* dY, const void* act, const float* o, const float* stats, const float* gamma, int B, int HW, int C, float eps,
                               void* dpre_out, float* scratch_part, float* scratch_sums, float* dgamma, float* dbeta, void* d_o, void* stream) {
   if (!dY || !act || !o || !stats || !gamma || !scratch_part || !scratch_sums || !d_o) { snprintf(q_err, sizeof q_err, "gq_bn_relu_bwd: bad argument"); return -1; }
+  if (C % 8) { snprintf(q_err, sizeof q_err, "gq_bn_relu_bwd: C must be a multiple of 8"); return -1; }
   cudaStream_t st = (cudaStream_t)stream;
   const int rows = B * HW, rpc = 128, nparts = (rows + rpc - 1) / rpc;
   k_bn_bwd_reduce<<<nparts, 256, 0, st>>>((const bf16*)dY, (const bf16*)act, o, stats, rows, C, HW, eps, rpc, (bf16*)dpre_out, scratch_part);
   k_bn_bwd_sums<<<(C + 3) / 4, 128, 0, st>>>(scratch_part, nparts, C, scratch_sums, dgamma, dbeta);
   const size_t n = (size_t)rows * C;
-  if (C % 8 == 0)
-    k_bn_bwd_apply8<<<(unsigned)((n / 8 + 255) / 256), 256, 0, st>>>((const bf16*)dY, (const bf16*)act, o, stats, gamma, scratch_sums, n / 8, C, HW, 1.f / (float)rows, eps,
-                                                                       (bf16*)d_o);
-  else
-    k_bn_bwd_apply<<<(unsigned)((n + 255) / 256), 256, 0, st>>>((const bf16*)dY, (const bf16*)act, o, stats, gamma, scratch_sums, n, C, HW, 1.f / (float)rows, eps,
-                                                                  (bf16*)d_o);
+  k_bn_bwd_apply8<<<(unsigned)((n / 8 + 255) / 256), 256, 0, st>>>((const bf16*)dY, (const bf16*)act, o, stats, gamma, scratch_sums, n / 8, C, HW, 1.f / (float)rows, eps,
+                                                                     (bf16*)d_o);
   QCK(cudaGetLastError());
   return 0;
 }
 
 // ------------------------------------------------------------------------------------------------ weight gradient on wgmma
-// The same contraction as k_wgrad as a tensor-core GEMM:  D[co][ci] (one filter tap, one image) = sum over pixels p of dY[p][co] * X[p + tap][ci],
+// dW[co][tap][ci] = sum over images b and pixels p of dY[b,p,co] * X[b, p + tap, ci]  (zero outside the image), as a tensor-core GEMM:
+// D[co][ci] (one filter tap, one image) = sum over pixels p of dY[p][co] * X[p + tap][ci],
 // i.e. M = 128 output channels, N = BLOCK_N input channels, K = pixels.  Both operands are pixel-major in memory ([pixel][channel], NHWC), so
 // with K = pixels they are **MN-major** wgmma operands: a shared-memory tile is K rows (pixels) of 128 bytes (64 channels), 8 rows = one
 // 1024-byte swizzle atom - exactly the image a 128-byte-swizzled TMA box of [64 channels x 128 pixels] leaves.  Canonical MN-major
@@ -510,7 +401,7 @@ extern "C" int gq_bn_relu_bwd(const void* dY, const void* act, const float* o, c
 //   A = dY: 3-D tiled map [Cout][H*W][B], box 64 x 128 x 1 - rows past the end of the image are out of bounds and read as zeros, so the
 //           last k-step of an image contributes nothing for them whatever the X load returns there;
 //   B = X : the forward's im2col-mode map (tap passed as offsets, zero fill = convolution padding): 128 consecutive output positions.
-// grid (ceil(Cout / 128), Cin / BLOCK_N, taps * B); split-K over the images like k_wgrad (partials [B][Cout][taps][Cin], summed in image
+// grid (ceil(Cout / 128), Cin / BLOCK_N, taps * B); split-K over the images (partials [B][Cout][taps][Cin], summed in image
 // order by k_reduce_rows: deterministic).  Roles as in k_conv_wgmma: warp 8 lane 0 TMA producer, warpgroup g = 0, 1 multiplies and stores
 // output channels co0 + 64 g .. co0 + 64 g + 63 (its own dY box).
 __device__ __forceinline__ void tma_load_3d(uint32_t dst_smem_addr, const CUtensorMap* tmap, int c0, int c1, int c2, uint64_t* bar) {
@@ -608,11 +499,13 @@ static int make_dy_tmap(CUtensorMap* m, const void* dy, int B, int HW, int Cout)
   if (r != CUDA_SUCCESS) { snprintf(q_err, sizeof q_err, "cuTensorMapEncodeTiled (dY) failed (%d)", (int)r); return -3; }
   return 0;
 }
-// -> 0 launched, 1 not available on this driver (caller uses k_wgrad), < 0 error
+// -> 0 launched, < 0 error (q_err set)
 static int launch_wgrad_tc(cudaStream_t st, const void* dY, const void* x, float* part, int B, int H, int W, int Cin, int Cout, int ks) {
   alignas(64) CUtensorMap tdy, tx;
   memset(&tdy, 0, sizeof tdy); memset(&tx, 0, sizeof tx);
-  if (make_dy_tmap(&tdy, dY, B, H * W, Cout) != 0 || make_act_tmap_im2col(&tx, x, B, H, W, Cin, ks) != 0) return 1;
+  int r = make_dy_tmap(&tdy, dY, B, H * W, Cout);
+  if (r == 0) r = make_act_tmap_im2col(&tx, x, B, H, W, Cin, ks);
+  if (r) return r;
   const int taps = ks * ks;
 #define LAUNCH_WT(BN_, ST_)                                                                                                   \
   do {                                                                                                                        \
@@ -632,15 +525,8 @@ extern "C" int gq_conv_wgrad(const void* dY, const void* x, float* scratch_part,
   if (!dY || !x || !scratch_part || !dW || (ks != 1 && ks != 3) || Cin % 64 || Cout % 64) { snprintf(q_err, sizeof q_err, "gq_conv_wgrad: bad argument"); return -1; }
   cudaStream_t st = (cudaStream_t)stream;
   const int taps = ks * ks;
-  // wgmma path by default (GQ_WGRAD_TC=0: the CUDA-core kernel, kept as the A/B partner and for drivers without the tensor-map encoders)
-  const char* e_tc = getenv("GQ_WGRAD_TC");  // (read per call: the parity test switches between the two kernels inside one process)
-  const int use_tc = (e_tc && atoi(e_tc) == 0) ? 0 : 1;
-  int r = use_tc ? launch_wgrad_tc(st, dY, x, scratch_part, B, H, W, Cin, Cout, ks) : 1;
-  if (r < 0) return r;
-  if (r == 1) {
-    dim3 grid(Cout / WG_T, Cin / WG_T, taps * B);
-    k_wgrad<<<grid, 256, 0, st>>>((const bf16*)dY, (const bf16*)x, scratch_part, H, W, Cin, Cout, ks);
-  }
+  const int r = launch_wgrad_tc(st, dY, x, scratch_part, B, H, W, Cin, Cout, ks);
+  if (r) return r;
   const size_t n = (size_t)Cout * taps * Cin;
   k_reduce_rows<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(scratch_part, dW, B, n);
   QCK(cudaGetLastError());
@@ -657,9 +543,9 @@ extern "C" int gq_conv_first_wgrad(const void* dY, const float* x, float* scratc
   return 0;
 }
 extern "C" int gq_maxpool_bwd(const void* x, const void* dY, void* dX, int B, int H, int W, int C, void* stream) {
+  if (C % 8) { snprintf(q_err, sizeof q_err, "gq_maxpool_bwd: C must be a multiple of 8"); return -1; }
   const size_t n = (size_t)B * H * W * C;
-  if (C % 8 == 0) k_maxpool_bwd8<<<(unsigned)((n / 8 + 255) / 256), 256, 0, (cudaStream_t)stream>>>((const bf16*)x, (const bf16*)dY, (bf16*)dX, B, H, W, C);
-  else k_maxpool_bwd<<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>((const bf16*)x, (const bf16*)dY, (bf16*)dX, B, H, W, C);
+  k_maxpool_bwd8<<<(unsigned)((n / 8 + 255) / 256), 256, 0, (cudaStream_t)stream>>>((const bf16*)x, (const bf16*)dY, (bf16*)dX, B, H, W, C);
   QCK(cudaGetLastError());
   return 0;
 }

@@ -23,7 +23,7 @@ import numpy as np
 _HERE = os.path.dirname(os.path.abspath(__file__))
 QLIB_PATH = os.path.join(_HERE, "csrc", "libgrasp_qnet.so")
 _QLIB = None
-QSYMBOLS = ["gq_last_error", "gq_version", "gq_conv_partials_floats", "gq_conv_tc", "gq_conv_tc_block_out", "gq_conv_first", "gq_maxpool", "gq_bn_act", "gq_upsample2x", "gq_head", "gq_head_up2", "gq_argmax", "gq_obs_to_state", "gq_obs_to_state_train", "gq_conv_tc_fused",
+QSYMBOLS = ["gq_last_error", "gq_version", "gq_conv_partials_floats", "gq_conv_tc", "gq_conv_tc_block_out", "gq_conv_first", "gq_maxpool", "gq_bn_act", "gq_upsample2x", "gq_head_up2", "gq_argmax", "gq_obs_to_state", "gq_obs_to_state_train", "gq_conv_tc_fused",
             "gq_obs_to_state_keyed", "gq_sample_actions"]
 
 
@@ -45,7 +45,6 @@ def load_qnet_library():
         L.gq_maxpool.argtypes = [P, P, I, I, I, I, P]
         L.gq_bn_act.argtypes = [P, P, P, P, P, P, I, I, I, F, P]
         L.gq_upsample2x.argtypes = [P, P, I, I, I, I, P]
-        L.gq_head.argtypes = [P, P, P, P, I, I, I, P]
         L.gq_head_up2.argtypes = [P, P, P, P, P, I, I, I, I, P]
         L.gq_argmax.argtypes = [P, I, I, P, P, P]
         L.gq_obs_to_state.argtypes = [P, P, F, P, P, I, I, P]
@@ -169,17 +168,9 @@ class QNetForward:
                          b3=sd[f"{name}.conv3.bias"].contiguous(), g1=sd[f"{name}.bn1.weight"].contiguous(), be1=sd[f"{name}.bn1.bias"].contiguous(),
                          g2=sd[f"{name}.bn2.weight"].contiguous(), be2=sd[f"{name}.bn2.bias"].contiguous(), cin=cin, cout=cout)
             self.blocks.append(b)
-        # BasicBlock tail: shortcut conv + BN-apply of the main branch + add + ReLU in one kernel (GQ_FUSE_TAIL=0: separate kernels)
-        self.fuse_tail = os.environ.get("GQ_FUSE_TAIL", "1") != "0"
-        # network tail: head on the 100x100 map, then up-sample its 6 planes (GQ_FUSE_HEAD=0: up-sample 64 channels, then the head)
-        self.fuse_head = os.environ.get("GQ_FUSE_HEAD", "1") != "0"
         self.w_head = sd["1.C1.weight"].reshape(self.A, 64).contiguous()
         self.b_head = sd["1.C1.bias"].contiguous()
         self.launches = 0
-        # GQ_GRAPH=1: the ~110 launches of one chunk captured once per input shape in a CUDA graph and replayed (static input / output
-        # buffers; tensor maps and pointers are baked into the graph).  Off by default: see DESIGN.md for the measurement.
-        self.use_graph = os.environ.get("GQ_GRAPH", "0") == "1"
-        self._graphs = {}
 
     def _ck(self, r, what):
         if r != 0:
@@ -234,10 +225,7 @@ class QNetForward:
         o1, s1 = self.conv_tc(x, blk["w1"], None, B, H, W, cin, cout, 3, True)
         a1 = self.bn_act(o1, s1, blk["g1"], blk["be1"], None, B, H * W, cout)
         o2, s2 = self.conv_tc(a1, blk["w2"], None, B, H, W, cout, cout, 3, True)
-        if self.fuse_tail:
-            return self.conv_tc_block_out(x, blk["w3"], blk["b3"], o2, s2, blk["g2"], blk["be2"], B, H, W, cin, cout, 1)
-        idn, _ = self.conv_tc(x, blk["w3"], blk["b3"], B, H, W, cin, cout, 1, False)
-        return self.bn_act(o2, s2, blk["g2"], blk["be2"], idn, B, H * W, cout)
+        return self.conv_tc_block_out(x, blk["w3"], blk["b3"], o2, s2, blk["g2"], blk["be2"], B, H, W, cin, cout, 1)
 
     def maxpool(self, x, B, H, W, Cc):
         t = self.torch
@@ -268,46 +256,17 @@ class QNetForward:
         x = self.upsample(x.view(B, h2, w2, 128), B, h2, w2, 128)   # -> 100
         x = self.basic_block(x, self.blocks[5], B, 2 * h2, 2 * w2)  # 1.RB3 128->64
         q = t.empty((B, self.A, 4 * h2, 4 * w2), dtype=t.float32, device=self.dev)
-        if self.fuse_head:
-            z = t.empty((B, self.A, 2 * h2, 2 * w2), dtype=t.float32, device=self.dev)
-            self._ck(self.L.gq_head_up2(self._p(x), self._p(self.w_head), self._p(self.b_head), self._p(z), self._p(q), B, 2 * h2, 2 * w2, self.A, self._stream()),
-                     "gq_head_up2")
-            return q
-        x = self.upsample(x.view(B, 2 * h2, 2 * w2, 64), B, 2 * h2, 2 * w2, 64)  # -> 200
-        HW = 16 * h2 * w2
-        self._ck(self.L.gq_head(self._p(x), self._p(self.w_head), self._p(self.b_head), self._p(q), B, HW, self.A, self._stream()), "gq_head")
+        z = t.empty((B, self.A, 2 * h2, 2 * w2), dtype=t.float32, device=self.dev)
+        self._ck(self.L.gq_head_up2(self._p(x), self._p(self.w_head), self._p(self.b_head), self._p(z), self._p(q), B, 2 * h2, 2 * w2, self.A, self._stream()),
+                 "gq_head_up2")
         return q
 
     def forward(self, state):
         """state [B,4,H,W] f32 on the device -> Q [B,A,H,W] f32 (sigmoid), chunked to bound activation memory"""
         t = self.torch
         state = state.to(self.dev, t.float32).contiguous()
-        fn = self._forward_chunk_graphed if self.use_graph else self._forward_chunk
-        outs = [fn(state[i:i + self.max_batch]) for i in range(0, state.shape[0], self.max_batch)]
+        outs = [self._forward_chunk(state[i:i + self.max_batch]) for i in range(0, state.shape[0], self.max_batch)]
         return outs[0] if len(outs) == 1 else t.cat(outs, dim=0)
-
-    def _forward_chunk_graphed(self, state):
-        t = self.torch
-        key = tuple(state.shape)
-        g = self._graphs.get(key)
-        if g is None:
-            sin = state.clone()
-            cur = t.cuda.current_stream(self.dev)
-            side = t.cuda.Stream(self.dev)
-            side.wait_stream(cur)
-            with t.cuda.stream(side):  # warm-up outside the capture (function attributes, driver entry points, allocator)
-                self._forward_chunk(sin)
-            cur.wait_stream(side)
-            n0 = self.launches
-            graph = t.cuda.CUDAGraph()
-            with t.cuda.graph(graph):
-                sout = self._forward_chunk(sin)
-            g = self._graphs[key] = (graph, sin, sout, self.launches - n0)
-        graph, sin, sout, nl = g
-        sin.copy_(state)
-        graph.replay()
-        self.launches += nl
-        return sout.clone()
 
     def obs_to_state(self, obs, depth_threshold=1.1):
         """batched deterministic transform_observation: obs dict of device tensors (rgb u8 [B,H,W,3], depth f32 [B,H,W]) -> [B,4,H,W] f32.

@@ -111,11 +111,12 @@ def _conv_case(B, ks, cin, cout, H, W):
                                                # trainer's): 100 x 100 and 50 x 50 maps end in a partial 128-pixel k-step
                                                _conv_case(12, 3, 64, 128, 100, 100), _conv_case(15, 3, 128, 256, 50, 50), _conv_case(12, 3, 256, 512, 50, 50),
                                                _conv_case(15, 1, 512, 256, 50, 50), _conv_case(15, 3, 128, 64, 100, 100)])
-@pytest.mark.parametrize("tc", [1, 0])
-def test_wgrad_and_dgrad_match_autograd(learner, B, ks, cin, cout, H, W, tc, monkeypatch):
-    """tc = 1: the wgmma weight-gradient kernel (default); tc = 0: its CUDA-core A/B partner (GQ_WGRAD_TC=0).  Reference: autograd of
-    F.conv2d in float64 on the same bf16 values"""
-    monkeypatch.setenv("GQ_WGRAD_TC", str(tc))
+@pytest.mark.parametrize("nan_prefill", [1, 0])
+def test_wgrad_and_dgrad_match_autograd(learner, B, ks, cin, cout, H, W, nan_prefill):
+    """the wgmma weight-gradient kernel and the dgrad through the forward convolution.  Reference: autograd of F.conv2d in float64 on
+    the same bf16 values.  The weight gradient's scratch and output buffers are, before the call:
+    nan_prefill = 1: NaN, so that every split-K partial and every element of dW must be written by the call;
+    nan_prefill = 0: the result of an identical earlier call, which the new result must equal bit for bit (partials summed in fixed order)"""
     g = torch.Generator(device="cuda").manual_seed(1)
     x = _bf(torch.randn((B, H, W, cin), generator=g, device="cuda"))
     dY = _bf(torch.randn((B, H, W, cout), generator=g, device="cuda"))
@@ -128,7 +129,19 @@ def test_wgrad_and_dgrad_match_autograd(learner, B, ks, cin, cout, H, W, tc, mon
     # wgrad
     part = torch.empty(B * cout * ks * ks * cin, dtype=torch.float32, device="cuda")
     dW = torch.empty((cout, ks * ks, cin), dtype=torch.float32, device="cuda")
-    learner._ck(learner.L.gq_conv_wgrad(learner._p(dY), learner._p(x), learner._p(part), learner._p(dW), B, H, W, cin, cout, ks, learner._st()), "gq_conv_wgrad")
+
+    def wgrad():
+        learner._ck(learner.L.gq_conv_wgrad(learner._p(dY), learner._p(x), learner._p(part), learner._p(dW), B, H, W, cin, cout, ks, learner._st()), "gq_conv_wgrad")
+
+    if nan_prefill:
+        part.fill_(float("nan"))
+        dW.fill_(float("nan"))
+    else:
+        wgrad()
+        first = dW.clone()
+    wgrad()
+    if not nan_prefill:
+        assert torch.equal(dW, first)
     e_w = rel(dW.view(cout, ks, ks, cin).permute(0, 3, 1, 2), wr.grad)
     # dgrad through the forward convolution kernel with flipped / transposed weights
     wT = wb.float().flip(2, 3).permute(1, 2, 3, 0).contiguous().to(torch.bfloat16)
@@ -184,6 +197,12 @@ def test_bn_relu_backward_matches_autograd(learner):
     assert rel(d_o.float(), orf.grad) < 6e-3          # bf16 output
     assert rel(dg, gr.grad) < 1e-4 and rel(db, br.grad) < 1e-4
     assert rel(dpre.float(), dY.float() * (act.float() > 0)) == 0.0
+    # the kernels move 8 channels per thread: other channel counts are refused
+    o12 = torch.zeros((B, HW, 12), device="cuda")
+    y12, d12 = torch.zeros((B, HW, 12), dtype=torch.bfloat16, device="cuda"), torch.empty((B, HW, 12), dtype=torch.bfloat16, device="cuda")
+    with pytest.raises(RuntimeError, match="gq_bn_relu_bwd: C must be a multiple of 8"):
+        learner._ck(learner.L.gq_bn_relu_bwd(learner._p(y12), learner._p(y12), learner._p(o12), learner._p(stats), learner._p(gamma), B, HW, 12, 1e-5, None,
+                                             learner._p(part), learner._p(sums), None, None, learner._p(d12), learner._st()), "gq_bn_relu_bwd")
 
 
 @gpu
@@ -199,6 +218,11 @@ def test_pool_upsample_backward_match_autograd(learner):
     dX = torch.empty((B, H, W, Cc), dtype=torch.bfloat16, device="cuda")
     learner._ck(learner.L.gq_maxpool_bwd(learner._p(x), learner._p(dY), learner._p(dX), B, H, W, Cc, learner._st()), "gq_maxpool_bwd")
     assert rel(dX.float().permute(0, 3, 1, 2), xr.grad) < 4e-3
+    # 8 channels per thread: other channel counts are refused
+    x12, dY12 = torch.zeros((B, H, W, 12), dtype=torch.bfloat16, device="cuda"), torch.zeros((B, OH, OW, 12), dtype=torch.bfloat16, device="cuda")
+    dX12 = torch.empty((B, H, W, 12), dtype=torch.bfloat16, device="cuda")
+    with pytest.raises(RuntimeError, match="gq_maxpool_bwd: C must be a multiple of 8"):
+        learner._ck(learner.L.gq_maxpool_bwd(learner._p(x12), learner._p(dY12), learner._p(dX12), B, H, W, 12, learner._st()), "gq_maxpool_bwd")
     # bilinear x2, align_corners=True
     zr = torch.randn((B, Cc, H, W), generator=g, device="cuda").requires_grad_(True)
     up = F.interpolate(zr, scale_factor=2, mode="bilinear", align_corners=True)

@@ -53,7 +53,8 @@ int ge_destroy(ge_handle h);
  * overflow row since ge_create (synchronises the engine's stream; saturates at INT_MAX).  Both builds read GE_HCAP at ge_create (hcap,
  * CTA-per-env build: from Σ tree blocks + 6 maxcon + 64 up to hfull; warp-per-env build: from the larger of Σ tree blocks and
  * 6 maxcon + 6 nbody up to hfull); both also read GE_MAXCON (contact capacity, 16..512; the default hcap and the smallest GE_HCAP
- * follow it).  A value outside its range is ignored, so size 6 / 10 tell what was used. */
+ * follow it).  A value outside its range is ignored, so size 6 / 10 tell what was used.  14 bytes R of one environment state record
+ * (ge_snapshot, below). */
 int ge_size(ge_handle h, int what);
 
 /* MujocoEnv.set_state + controller re-sync, as GraspEnv.reset_model does (GraspingEnv.py:466-470):
@@ -136,6 +137,40 @@ int ge_debug_forward(ge_handle h, int env, const char* field, double* out /*[hos
 
 /* counters: kernels launched by this handle since creation, and sub-step kernel launches among them */
 int ge_counters(ge_handle h, int64_t* kernel_launches, int64_t* substep_launches);
+
+/* Environment state records: save, restore and copy the whole state of environments, mid-movement or mid-program included.  The
+ * reference's counterpart is pickling an MjSim together with its controller and GraspEnv objects; ge_set_state is its reset_model and
+ * clears the warm start, the gains and any pending command, so it cannot resume a trajectory.
+ *
+ * One record per env, R = ge_size(h, 14) bytes, a multiple of 128; records of one call are packed back to back ([n, R]).  Format "GES1",
+ * little-endian, offsets in bytes:
+ *   0   u32  magic 0x31534547 ("GES1")        4  u32  R        8  u64  model fingerprint = FNV-1a-64 of the model blob bytes
+ *   16  f64  qpos[nq], qvel[nv], qaccws[nv] (the Newton warm start), ctl[32] (PID target[8] last_input[8] kp[8] ctrl[8]),
+ *            cmd_tol, prog_coords[3], prog_table
+ *   then i64 substeps (sim.step() calls since creation: the env's clock, MuJoCo's `time`)
+ *   then i32 cmd_active, cmd_mask, cmd_maxsteps, cmd_steps, cmd_result, prog_phase, prog_rot, prog_grasp, prog_aux, prog_info[12],
+ *            status, reward (u8 widened), then zeros up to R.
+ * Not part of a record, on purpose:
+ *   - the scheduling words of the sub-step kernel (lock, owed, done, ticket) and ge_run's busy counter: they belong to one launch.  Between
+ *     launches every lock and owed count is 0, done is reset at the start of each launch and ticket only orders the tasks of a launch
+ *     (relative to a base the host keeps), so they carry nothing about an env from one call to the next;
+ *   - the Hessian overflow rows and the workspace flag that says a build uses them: scratch of one Newton Hessian build, written before
+ *     they are read within that build;
+ *   - the engine's count of builds that used the overflow row (ge_size 13): a statistic of the engine, not of an environment.
+ * A record does not depend on the workspace layout, so it restores across GE_MAXCON / GE_HCAP settings and both library builds of one
+ * scene; it does depend on the model (fingerprint) and is refused by an engine of another scene.
+ *
+ * ge_snapshot: record i <- env envs[i] (envs [n] int32 [dev], or NULL for envs 0..N-1 with n = N); rec [n, R] [dev].  An index outside
+ * [0, N) gives an all-zero record, which ge_restore refuses.  Stream-ordered, no synchronisation.
+ * ge_restore: env e <- record row[e] of rec [n_rec, R] [dev] (row [N] int32 [dev]; -1 leaves env e alone; NULL = record e for env e).  A
+ * gather, so no env is written twice.  Checks every row and every record a row selects, synchronises the stream once, and returns
+ * GE_ERR_ARG (a row outside [-1, n_rec)) or GE_ERR_STATE (wrong magic, R or fingerprint) before writing anything: an engine that refuses
+ * a call is left bit for bit as it was.  A restored env continues exactly where the saved one stood, busy or not, with its saved substeps.
+ * ge_clone: env e <- the state env src[e] had before the call (src [N] int32 [dev], -1 = keep), so overlapping and permuting maps are
+ * fine.  Goes through an engine-owned scratch of N records (allocated at the first call, freed by ge_destroy); refuses like ge_restore. */
+int ge_snapshot(ge_handle h, const int32_t* envs, int n, void* rec);
+int ge_restore(ge_handle h, const void* rec, int n_rec, const int32_t* row);
+int ge_clone(ge_handle h, const int32_t* src);
 
 #ifdef __cplusplus
 }

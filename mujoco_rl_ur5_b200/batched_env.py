@@ -84,6 +84,7 @@ class BatchedGraspEnv:
         self.h2d_bytes_per_step = self._pin_action.numel() * 4
         self.d2h_bytes_per_step = self._pin_reward.numel()
         self.obs_bytes = n_envs * image_width * image_height * (3 + 4)  # rgb u8 x3 + depth f32
+        self._branch = None  # engine of evaluate_actions, created at its first call
 
     # ------------------------------------------------------------------ gym-like API
     def reset(self):
@@ -143,6 +144,68 @@ class BatchedGraspEnv:
         self.step_called += 1
         return self.current_observation, self._pin_reward.numpy().copy(), np.zeros(self.n_envs, bool), info
 
+    # ------------------------------------------------------------------ whole states (env_state.py)
+    def snapshot(self):
+        """EngineState of every env plus what this façade keeps beside the engine (current observation, step counter, episode), so
+        that a restored env's next `step` is the original's next `step`"""
+        s = self.engine.snapshot()
+        obs = None if self.current_observation is None else {k: v.clone() for k, v in self.current_observation.items()}
+        s.facade = {"observation": obs, "step_called": self.step_called, "episode": self.episode}
+        return s
+
+    def restore(self, s):
+        """puts back a `snapshot` (also one loaded with EngineState.load); raises EngineError, leaving everything as it was, for a
+        snapshot of another scene"""
+        self.engine.restore(s)
+        if s.facade is not None:
+            obs = s.facade.get("observation")
+            self.current_observation = None if obs is None else {k: v.to(self.engine.device).clone() for k, v in obs.items()}
+            self.step_called, self.episode = int(s.facade["step_called"]), int(s.facade["episode"])
+
+    def evaluate_actions(self, actions, max_branch_envs=4096):
+        """Grasp outcome of K candidate actions per env from the env's current state, without changing it: actions [N, K, 2] (pixel
+        index, rotation index as `step` takes them) -> (reward u8 [N, K], executed bool [N, K]) on the device.  Pixels turn into
+        world points as in `step` (the current observation's depth, bad-depth attempts skipped with reward 0); the N*K attempts run in
+        a second engine of the same scene, restored from this one's snapshot, at most `max_branch_envs` at a time.  Attempt (e, k) is
+        bit for bit what `step` would give with action k."""
+        t = self.torch
+        eng = self.engine
+        act = t.as_tensor(actions).to(device=eng.device, dtype=t.int32)
+        N, K = act.shape[0], act.shape[1]
+        if act.shape != (self.n_envs, K, 2) or K < 1 or max_branch_envs < 1:
+            raise ValueError(f"actions must be [{self.n_envs}, K, 2] and max_branch_envs >= 1, got {tuple(act.shape)}, {max_branch_envs}")
+        obs = self.current_observation if self.current_observation is not None else self.get_observation()
+        W, H = self.IMAGE_WIDTH, self.IMAGE_HEIGHT
+        ar = t.arange(N, device=eng.device)
+        coords = t.empty((N, K, 3), dtype=t.float64, device=eng.device)
+        for k in range(K):
+            x = act[:, k, 0] % W
+            y = t.div(act[:, k, 0], W, rounding_mode="floor")
+            d = obs["depth"][ar, y.long(), x.long()].contiguous()
+            coords[:, k] = eng.pixel_2_world(x.contiguous(), y.contiguous(), d, self.cam, W, H)
+        execute = ~((coords[..., 2] < 0.8) | (coords[..., 1] > -0.3))  # as in step
+        coords, rot, execute = coords.reshape(N * K, 3), act[..., 1].reshape(N * K), execute.reshape(N * K)
+        B = min(N * K, int(max_branch_envs))
+        if self._branch is None or self._branch.n_envs != B:
+            if self._branch is not None:
+                self._branch.close()
+            self._branch = BatchedEngine(self.blob, B, eng.device.index or 0)
+        br = self._branch
+        state = eng.snapshot()
+        reward = t.zeros(N * K, dtype=t.uint8, device=eng.device)
+        slot = t.arange(B, device=eng.device)
+        for j0 in range(0, N * K, B):
+            n = min(B, N * K - j0)
+            live = slot < n
+            rows = t.where(live, t.div(j0 + slot, K, rounding_mode="floor"), t.full_like(slot, -1))
+            br.restore(state, rows)
+            pad = lambda a: t.cat([a[j0:j0 + n], a[:B - n]]) if n < B else a[j0:j0 + n]
+            mask = pad(execute) & live
+            br.grasp(pad(coords).contiguous(), pad(rot).contiguous(), self.TABLE_HEIGHT, env_mask=mask.to(t.uint8))
+            br.run()
+            reward[j0:j0 + n] = (br.results()[2] * mask.to(t.uint8))[:n]
+        return reward.reshape(N, K), execute.reshape(N, K)
+
     def render(self, mode="rgb_array"):
         return self.get_observation()["rgb"]
 
@@ -154,3 +217,5 @@ class BatchedGraspEnv:
 
     def close(self):
         self.engine.close()
+        if self._branch is not None:
+            self._branch.close()

@@ -38,6 +38,9 @@ typedef void* vh;
   int ge_render_##suffix(vh, int, int, int, uint8_t*, float*);                                                                     \
   int ge_debug_forward_##suffix(vh, int, const char*, double*, int);                                                               \
   int ge_counters_##suffix(vh, int64_t*, int64_t*);                                                                                \
+  int ge_snapshot_##suffix(vh, const int32_t*, int, void*);                                                                        \
+  int ge_restore_##suffix(vh, const void*, int, const int32_t*);                                                                   \
+  int ge_clone_##suffix(vh, const int32_t*);                                                                                       \
   }
 DECL(smem)
 DECL(hbm)
@@ -100,5 +103,8 @@ int ge_pixel_2_world(ge_handle h, int cam, int w, int hh, const int32_t* px, con
 int ge_render(ge_handle h, int cam, int w, int hh, uint8_t* rgb, float* d) { CHECK_H; return FWD(ge_render_smem(h->h, cam, w, hh, rgb, d), ge_render_hbm(h->h, cam, w, hh, rgb, d)); }
 int ge_debug_forward(ge_handle h, int env, const char* f, double* out, int cap) { CHECK_H; return FWD(ge_debug_forward_smem(h->h, env, f, out, cap), ge_debug_forward_hbm(h->h, env, f, out, cap)); }
 int ge_counters(ge_handle h, int64_t* a, int64_t* b) { CHECK_H; return FWD(ge_counters_smem(h->h, a, b), ge_counters_hbm(h->h, a, b)); }
+int ge_snapshot(ge_handle h, const int32_t* e, int n, void* r) { CHECK_H; return FWD(ge_snapshot_smem(h->h, e, n, r), ge_snapshot_hbm(h->h, e, n, r)); }
+int ge_restore(ge_handle h, const void* r, int n, const int32_t* row) { CHECK_H; return FWD(ge_restore_smem(h->h, r, n, row), ge_restore_hbm(h->h, r, n, row)); }
+int ge_clone(ge_handle h, const int32_t* src) { CHECK_H; return FWD(ge_clone_smem(h->h, src), ge_clone_hbm(h->h, src)); }
 
 }  // extern "C"

@@ -58,4 +58,7 @@
 #define ge_render GE_API(ge_render)
 #define ge_debug_forward GE_API(ge_debug_forward)
 #define ge_counters GE_API(ge_counters)
+#define ge_snapshot GE_API(ge_snapshot)
+#define ge_restore GE_API(ge_restore)
+#define ge_clone GE_API(ge_clone)
 #define ge_engine GE_API(ge_engine)

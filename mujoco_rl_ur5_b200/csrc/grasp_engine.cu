@@ -414,6 +414,98 @@ __global__ void __launch_bounds__(GE_LANES) k_body_xpos(EnvArrays E, int n_env, 
   LANE_LOOP(i, 3 * m.nbody) xpos[(size_t)env * 3 * m.nbody + i] = ws[L.xpos + i];
 }
 
+// ---- environment state records (ge_snapshot / ge_restore / ge_clone; format in include/grasp_engine.h).  A record is `words` 8-byte
+// words: [0] magic | R << 32, [1] model fingerprint, then qpos, qvel, qaccws, ctl as raw f64 bits, then the tail: cmd_tol,
+// prog_coords[3], prog_table, substeps, and the 23 int fields two per word, zero padding to R.  One warp per env; the [N, nq] / [N, nv] /
+// [N, 32] rows are read and written lane-strided (coalesced), everything moves as 64-bit words, so a round trip is bit-exact.
+#define GE_REC_MAGIC 0x31534547u  // "GES1"
+#define GE_REC_NINT 23            // cmd_active cmd_mask cmd_maxsteps cmd_steps cmd_result prog_phase prog_rot prog_grasp prog_aux prog_info[12] status reward
+#define GE_REC_NTAIL (6 + (GE_REC_NINT + 1) / 2)
+__host__ __device__ inline int rec_words(int nq, int nv) { return (2 + nq + 2 * nv + 32 + GE_REC_NTAIL + 15) / 16 * 16; }  // R = 8 x this, a multiple of 128 B
+__device__ __forceinline__ int* rec_int_ptr(const EnvArrays& E, int env, int k) {
+  switch (k) {
+    case 0: return E.cmd_active + env; case 1: return E.cmd_mask + env; case 2: return E.cmd_maxsteps + env; case 3: return E.cmd_steps + env;
+    case 4: return E.cmd_result + env; case 5: return E.prog_phase + env; case 6: return E.prog_rot + env; case 7: return E.prog_grasp + env;
+    case 8: return E.prog_aux + env; case 21: return E.status + env;
+  }
+  return k >= 9 && k < 21 ? E.prog_info + 12 * env + (k - 9) : nullptr;
+}
+__device__ __forceinline__ unsigned rec_int_get(const EnvArrays& E, int env, int k) {
+  if (k == 22) return E.reward[env];
+  const int* p = rec_int_ptr(E, env, k);
+  return p ? (unsigned)*p : 0u;
+}
+__device__ __forceinline__ void rec_int_set(const EnvArrays& E, int env, int k, unsigned v) {
+  if (k == 22) { E.reward[env] = (unsigned char)v; return; }
+  if (int* p = rec_int_ptr(E, env, k)) *p = (int)v;
+}
+__device__ __forceinline__ unsigned long long rec_tail_get(const EnvArrays& E, int env, int t) {
+  if (t == 0) return __double_as_longlong(E.cmd_tol[env]);
+  if (t <= 3) return __double_as_longlong(E.prog_coords[3 * env + t - 1]);
+  if (t == 4) return __double_as_longlong(E.prog_table[env]);
+  if (t == 5) return (unsigned long long)E.substeps[env];
+  const int k = 2 * (t - 6);
+  return rec_int_get(E, env, k) | (unsigned long long)rec_int_get(E, env, k + 1) << 32;
+}
+__device__ __forceinline__ void rec_tail_set(const EnvArrays& E, int env, int t, unsigned long long w) {
+  if (t == 0) E.cmd_tol[env] = __longlong_as_double(w);
+  else if (t <= 3) E.prog_coords[3 * env + t - 1] = __longlong_as_double(w);
+  else if (t == 4) E.prog_table[env] = __longlong_as_double(w);
+  else if (t == 5) E.substeps[env] = (long long)w;
+  else { const int k = 2 * (t - 6); rec_int_set(E, env, k, (unsigned)w); if (k + 1 < GE_REC_NINT) rec_int_set(E, env, k + 1, (unsigned)(w >> 32)); }
+}
+// record i <- env envs[i] (envs NULL: env i).  An index outside [0, n_env) gives an all-zero record, which ge_restore rejects.
+__global__ void k_state_pack(EnvArrays E, int n_env, int nq, int nv, const int* envs, int n, unsigned long long fp, int words,
+                             unsigned long long* rec) {
+  const int i = blockIdx.x * blockDim.y + threadIdx.y, lane = threadIdx.x;
+  if (i >= n) return;
+  const int env = envs ? envs[i] : i;
+  unsigned long long* r = rec + (size_t)i * words;
+  if (env < 0 || env >= n_env) { for (int w = lane; w < words; w += 32) r[w] = 0; return; }
+  if (lane == 0) r[0] = GE_REC_MAGIC | (unsigned long long)(words * 8) << 32;
+  if (lane == 1) r[1] = fp;
+  unsigned long long* d = r + 2;
+  const unsigned long long *qpos = (const unsigned long long*)E.qpos + (size_t)env * nq, *qvel = (const unsigned long long*)E.qvel + (size_t)env * nv,
+                           *qacc = (const unsigned long long*)E.qaccws + (size_t)env * nv;
+  for (int k = lane; k < nq; k += 32) d[k] = qpos[k];
+  d += nq;
+  for (int k = lane; k < nv; k += 32) { d[k] = qvel[k]; d[nv + k] = qacc[k]; }
+  d += 2 * nv;
+  d[lane] = ((const unsigned long long*)E.ctl)[(size_t)env * 32 + lane];
+  d += 32;
+  const int ntail = words - (int)(d - r);
+  for (int t = lane; t < ntail; t += 32) d[t] = t < GE_REC_NTAIL ? rec_tail_get(E, env, t) : 0ULL;
+}
+// counts into bad[0] the rows (row[e], or e when row is NULL) outside [-1, n_rec) and into bad[1] the records a valid row points at whose
+// header is not this engine's (magic, size, fingerprint)
+__global__ void k_state_check(const unsigned long long* rec, int n_rec, int words, unsigned long long fp, const int* row, int n_env, int* bad) {
+  const int env = blockIdx.x * blockDim.y + threadIdx.y, lane = threadIdx.x;
+  if (env >= n_env) return;
+  const int r = row ? row[env] : env;
+  if (r < -1 || r >= n_rec) { if (lane == 0) atomicAdd(bad, 1); return; }
+  if (r < 0) return;
+  const unsigned long long want = lane == 0 ? (GE_REC_MAGIC | (unsigned long long)(words * 8) << 32) : fp;
+  const bool wrong = lane < 2 && rec[(size_t)r * words + lane] != want;
+  if (__ballot_sync(FULL, wrong) && lane == 0) atomicAdd(bad + 1, 1);
+}
+// env e <- record row[e] (row NULL: record e; -1: e untouched); rows and headers were checked by k_state_check
+__global__ void k_state_unpack(EnvArrays E, int n_env, int nq, int nv, const unsigned long long* rec, int words, const int* row) {
+  const int env = blockIdx.x * blockDim.y + threadIdx.y, lane = threadIdx.x;
+  if (env >= n_env) return;
+  const int ri = row ? row[env] : env;
+  if (ri < 0) return;
+  const unsigned long long* d = rec + (size_t)ri * words + 2;
+  unsigned long long *qpos = (unsigned long long*)E.qpos + (size_t)env * nq, *qvel = (unsigned long long*)E.qvel + (size_t)env * nv,
+                     *qacc = (unsigned long long*)E.qaccws + (size_t)env * nv;
+  for (int k = lane; k < nq; k += 32) qpos[k] = d[k];
+  d += nq;
+  for (int k = lane; k < nv; k += 32) { qvel[k] = d[k]; qacc[k] = d[nv + k]; }
+  d += 2 * nv;
+  ((unsigned long long*)E.ctl)[(size_t)env * 32 + lane] = d[lane];
+  d += 32;
+  if (lane < GE_REC_NTAIL) rec_tail_set(E, env, lane, d[lane]);
+}
+
 }  // namespace ge
 
 // ------------------------------------------------------------------------------------------------ host side
@@ -439,6 +531,9 @@ struct ge_engine {
   unsigned long long ticket_base;  // tasks issued by all previous launches
   int* d_nout; double* d_dbg;
   RenderCtx rctx;
+  unsigned long long fingerprint;  // FNV-1a-64 of the model blob: written into every state record, checked by ge_restore
+  int* d_check;                    // [2] rows / records k_state_check rejected
+  void* state_scratch;             // [n_envs, R] records of ge_clone, allocated at its first call
 };
 
 static const void* blob_find(const std::vector<char>& b, const char* name, int64_t* count) {
@@ -576,6 +671,9 @@ extern "C" int ge_create(const void* model_blob, size_t nbytes, int n_envs, int 
   ge_engine* h = new ge_engine();
   h->device = device; h->n_envs = n_envs; h->stream = (cudaStream_t)stream; h->launches = h->substep_launches = 0;
   h->hblob.assign((const char*)model_blob, (const char*)model_blob + nbytes);
+  h->fingerprint = 0xcbf29ce484222325ULL;
+  for (size_t i = 0; i < nbytes; i++) h->fingerprint = (h->fingerprint ^ (unsigned char)h->hblob[i]) * 0x100000001b3ULL;
+  h->state_scratch = nullptr;
   CK(cudaMalloc(&h->dblob, nbytes));
   CK(cudaMemcpy(h->dblob, model_blob, nbytes, cudaMemcpyHostToDevice));
   DevModel& m = h->hm;
@@ -752,7 +850,7 @@ extern "C" int ge_create(const void* model_blob, size_t nbytes, int n_envs, int 
   }
   E.gws = nullptr;
   if (h->lay.hcap < h->lay.hfull) { AL(E.gws, double, N * (size_t)h->lay.hfull); }
-  AL(h->d_nout, int, 1); AL(h->d_dbg, double, 1 << 16);
+  AL(h->d_nout, int, 1); AL(h->d_dbg, double, 1 << 16); AL(h->d_check, int, 2);
 #undef AL
   render_init(h->rctx, m, h->hblob.data());
   // initial state: qpos0 for every env, controller targets = current joint angles
@@ -782,7 +880,7 @@ extern "C" int ge_destroy(ge_handle h) {
   EnvArrays& E = h->E;
   void* ptrs[] = {E.qpos, E.qvel, E.qaccws, E.ctl, E.cmd_mask, E.cmd_maxsteps, E.cmd_steps, E.cmd_result, E.cmd_active, E.cmd_tol, E.prog_phase,
                   E.prog_rot, E.prog_grasp, E.prog_aux, E.prog_info, E.prog_coords, E.prog_table, E.reward, E.status, E.substeps, E.busy_count,
-                  h->d_nout, h->d_dbg, h->dblob, E.gws, E.lock, E.owed, E.done, E.ticket, h->lay.hovf_builds};
+                  h->d_nout, h->d_dbg, h->dblob, E.gws, E.lock, E.owed, E.done, E.ticket, h->lay.hovf_builds, h->d_check, h->state_scratch};
   for (void* p : ptrs) cudaFree(p);
   render_free(h->rctx);
   delete h;
@@ -795,6 +893,7 @@ extern "C" int ge_size(ge_handle h, int what) {
     case 0: return h->hm.nq; case 1: return h->hm.nv; case 2: return h->hm.nbody; case 3: return h->hm.ngeom; case 4: return h->hm.nu;
     case 5: return h->n_envs; case 6: return h->lay.maxcon; case 7: return h->lay.total_bytes; case 8: return h->wpb; case 9: return h->lay.ws_global;
     case 10: return h->lay.hcap; case 11: return h->lay.hfull; case 12: return h->groups_per_sm;
+    case 14: return 8 * rec_words(h->hm.nq, h->hm.nv);
     case 13: {  // Hessian builds that used the overflow row since ge_create (saturates at INT_MAX)
       unsigned long long n = 0;
       CK(cudaSetDevice(h->device));
@@ -1029,6 +1128,47 @@ extern "C" int ge_debug_forward(ge_handle h, int env, const char* field, double*
   if (n > cap) n = cap;
   CK(cudaMemcpy(out, h->d_dbg, sizeof(double) * n, cudaMemcpyDeviceToHost));
   return n;
+}
+// Environment state records.  None of these kernels reads the model or the workspace layout in __constant__ memory, so no bind().
+extern "C" int ge_snapshot(ge_handle h, const int32_t* envs, int n, void* rec) {
+  if (!h || n < 0 || (n > 0 && !rec) || (!envs && n != h->n_envs)) return fail(GE_ERR_ARG, "ge_snapshot: bad argument");
+  if (n == 0) return GE_OK;
+  CK(cudaSetDevice(h->device));
+  k_state_pack<<<(n + 3) / 4, dim3(32, 4), 0, h->stream>>>(h->E, h->n_envs, h->hm.nq, h->hm.nv, envs, n, h->fingerprint,
+                                                          rec_words(h->hm.nq, h->hm.nv), (unsigned long long*)rec);
+  h->launches++;
+  CK(cudaGetLastError());
+  return GE_OK;
+}
+// check every row and every record it points at, wait for the verdict, then (only if all is well) scatter the records into the env rows
+static int unpack_checked(ge_handle h, const void* rec, int n_rec, const int32_t* row, const char* who) {
+  const int words = rec_words(h->hm.nq, h->hm.nv), blocks = (h->n_envs + 3) / 4;
+  const unsigned long long* r = (const unsigned long long*)rec;
+  CK(cudaMemsetAsync(h->d_check, 0, 2 * sizeof(int), h->stream));
+  k_state_check<<<blocks, dim3(32, 4), 0, h->stream>>>(r, n_rec, words, h->fingerprint, row, h->n_envs, h->d_check);
+  h->launches++;
+  CK(cudaGetLastError());
+  int bad[2] = {0, 0};
+  CK(cudaMemcpyAsync(bad, h->d_check, sizeof bad, cudaMemcpyDeviceToHost, h->stream));
+  CK(cudaStreamSynchronize(h->stream));
+  if (bad[0]) return fail(GE_ERR_ARG, "%s: record row outside [-1, number of records)", who);
+  if (bad[1]) return fail(GE_ERR_STATE, "%s: not a state record of this scene (magic, record size or model fingerprint differ)", who);
+  k_state_unpack<<<blocks, dim3(32, 4), 0, h->stream>>>(h->E, h->n_envs, h->hm.nq, h->hm.nv, r, words, row);
+  h->launches++;
+  CK(cudaGetLastError());
+  return GE_OK;
+}
+extern "C" int ge_restore(ge_handle h, const void* rec, int n_rec, const int32_t* row) {
+  if (!h || n_rec < 0 || (n_rec > 0 && !rec)) return fail(GE_ERR_ARG, "ge_restore: bad argument");
+  CK(cudaSetDevice(h->device));
+  return unpack_checked(h, rec, n_rec, row, "ge_restore");
+}
+extern "C" int ge_clone(ge_handle h, const int32_t* src) {
+  if (!h || !src) return fail(GE_ERR_ARG, "ge_clone: bad argument");
+  CK(cudaSetDevice(h->device));
+  if (!h->state_scratch) CK(cudaMalloc(&h->state_scratch, (size_t)h->n_envs * 8 * rec_words(h->hm.nq, h->hm.nv)));
+  int r = ge_snapshot(h, nullptr, h->n_envs, h->state_scratch);
+  return r ? r : unpack_checked(h, h->state_scratch, h->n_envs, src, "ge_clone");
 }
 extern "C" int ge_counters(ge_handle h, int64_t* kernel_launches, int64_t* substep_launches) {
   if (!h) return GE_ERR_ARG;

@@ -17,6 +17,7 @@ SYMBOLS = [
     "ge_last_error", "ge_version", "ge_create", "ge_destroy", "ge_size", "ge_set_state", "ge_get_state", "ge_get_body_xpos",
     "ge_set_gain", "ge_set_targets", "ge_get_targets", "ge_move_group", "ge_move_ee", "ge_stay", "ge_grasp", "ge_run", "ge_run_async", "ge_get_results",
     "ge_get_grasp_info", "ge_get_status", "ge_get_busy", "ge_set_ctrl", "ge_get_ctrl", "ge_step_open_loop", "ge_ik", "ge_pixel_2_world", "ge_render", "ge_debug_forward", "ge_counters",
+    "ge_snapshot", "ge_restore", "ge_clone",
 ]
 GROUPS = {"All": 0x7F, "Arm": 0x1F, "Gripper": 0x40}
 MOVE_RESULT = {0: "", 1: "success", 2: "max. steps reached: {}", 3: "No valid joint angles received, could not move EE to position."}
@@ -64,6 +65,9 @@ def load_library():
         L.ge_render.argtypes = [P, C.c_int, C.c_int, C.c_int, P, P]
         L.ge_debug_forward.argtypes = [P, C.c_int, C.c_char_p, C.POINTER(C.c_double), C.c_int]
         L.ge_counters.argtypes = [P, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
+        L.ge_snapshot.argtypes = [P, P, C.c_int, P]
+        L.ge_restore.argtypes = [P, P, C.c_int, P]
+        L.ge_clone.argtypes = [P, P]
         _LIB = L
     return _LIB
 
@@ -93,6 +97,7 @@ class BatchedEngine:
         self.n_envs = int(n_envs)
         self.nq, self.nv, self.nbody, self.ngeom, self.nu = [self.L.ge_size(h, k) for k in range(5)]
         self.smem_bytes = self.L.ge_size(h, 7)
+        self._blob, self._fingerprint = blob, None
 
     def size(self, what):
         """ge_size: 0 nq, 1 nv, 2 nbody, 3 ngeom, 4 nu, 5 n_envs, 6 max contacts, 7 workspace bytes per env, 8 envs per CTA,
@@ -141,6 +146,50 @@ class BatchedEngine:
         qvel = t.empty((self.n_envs, self.nv), dtype=t.float64, device=self.device)
         self._ck(self.L.ge_get_state(self.h, _ptr(qpos), _ptr(qvel)), "ge_get_state")
         return qpos, qvel
+
+    # ------------------------------------------------------------------ whole environment states (env_state.py, format "GES1")
+    @property
+    def state_bytes(self):
+        """bytes of one environment state record (ge_size 14)"""
+        return self.size(14)
+
+    @property
+    def fingerprint(self):
+        """FNV-1a-64 of the model blob, as the engine writes it into every record"""
+        if self._fingerprint is None:
+            from .env_state import fingerprint
+
+            self._fingerprint = fingerprint(self._blob)
+        return self._fingerprint
+
+    def snapshot(self, envs=None):
+        """EngineState with one record per env of `envs` (indices, default all), on this engine's device"""
+        from .env_state import EngineState
+
+        t = self.torch
+        ids = None if envs is None else self._dev(envs, t.int32).reshape(-1)
+        n = self.n_envs if ids is None else ids.numel()
+        rec = t.empty((n, self.state_bytes), dtype=t.uint8, device=self.device)
+        self._ck(self.L.ge_snapshot(self.h, _ptr(ids), n, _ptr(rec)), "ge_snapshot")
+        self._keep = ids
+        return EngineState(rec, self.nq, self.nv, self.fingerprint)
+
+    def restore(self, state, rows=None):
+        """env e <- record rows[e] of `state` (-1: leave env e alone; default: record e).  Raises EngineError, with the engine left
+        unchanged, for a record of another scene (GE_ERR_STATE) or a row outside [-1, len(state))"""
+        t = self.torch
+        if state.record_bytes != self.state_bytes:  # the library reads [n, R] records with its own R: refuse before it reads
+            raise EngineError(f"ge_restore refused: records of {state.record_bytes} bytes, this scene's are {self.state_bytes}")
+        rec = state.data.to(self.device).contiguous()
+        rows = None if rows is None else self._dev(rows, t.int32).reshape(self.n_envs)
+        self._ck(self.L.ge_restore(self.h, _ptr(rec), len(state), _ptr(rows)), "ge_restore")
+        self._keep = (rec, rows)
+
+    def clone(self, src):
+        """env e <- the state env src[e] had before the call (-1: keep); src [N]"""
+        src = self._dev(src, self.torch.int32).reshape(self.n_envs)
+        self._ck(self.L.ge_clone(self.h, _ptr(src)), "ge_clone")
+        self._keep = src
 
     def body_xpos(self):
         t = self.torch

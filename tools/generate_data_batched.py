@@ -4,8 +4,10 @@ epsilon-greedy actions from the Q-network, every (state, flat action, reward) wr
 (`Data/grasping_data_{k}.pt`, 12 transitions each; mujoco_rl_ur5_b200/offline_data.py) so that the reference's
 `Offline RL/train.py` / `grasping_dataset.py` read them unchanged.
 
-  python tools/generate_data_batched.py --envs 256 --episodes 2 --steps 10 --out Data [--weights ckpt.pt] [--eps 0.3]
+  python tools/generate_data_batched.py --envs 256 --episodes 2 --steps 10 --out Data [--weights ckpt.pt] [--eps 0.3] [--branches K]
 Needs a GPU (no CPU fallback).  One `add` = N transitions; episodes reset all environments (GraspingEnv.py:409-477).
+--branches K > 1: every step also labels K - 1 random table actions (BatchedGreedyAgent.random_table_actions) from the same state with
+BatchedGraspEnv.evaluate_actions, so one settled scene and one observation give K labelled transitions per env.
 """
 import argparse
 import os
@@ -24,6 +26,7 @@ def main():
     ap.add_argument("--weights", default=None, help="checkpoint written by the reference agent (key model_state_dict) or a bare state_dict")
     ap.add_argument("--scene", default="A")
     ap.add_argument("--seed", type=int, default=122)  # generate_data.py:16
+    ap.add_argument("--branches", type=int, default=1, help="labelled transitions per env and step (1 + K-1 random table actions)")
     args = ap.parse_args()
     import torch
 
@@ -42,8 +45,14 @@ def main():
         obs = env.reset()
         for _ in range(args.steps):
             act, _ = agent.epsilon_greedy(obs, args.eps)
+            extra = None
+            if args.branches > 1:  # labelled before the step: the extra attempts start from the state the observation shows
+                extra = torch.stack([agent.random_table_actions(obs) for _ in range(args.branches - 1)], dim=1)
+                extra_reward, _ = env.evaluate_actions(extra)
             nxt, reward, done, info = env.step(act)
             rec.add(obs, act, reward)
+            for k in range(args.branches - 1):
+                rec.add(obs, extra[:, k], extra_reward[:, k])
             obs = nxt
         print(f"episode {ep + 1}: rewards so far {dict(rec.reward_counter)}, {len(rec.files)} files")
     files = rec.close()

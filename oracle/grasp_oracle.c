@@ -89,6 +89,12 @@ typedef struct {
   int dim, geom1, geom2;
 } Contact;
 
+/* "boxbox" diagnostics, one record of BBX_W doubles per col_box_box call of the last collision stage: geom1, geom2, outcome
+ * (0 separated, 1 face contact, 2 edge-edge), the reference box (1, 2; 0 unless a face contact), the best face axis (0-5),
+ * face axes whose SAT separation equals the best one bit for bit (1: no tie), edge axes with 0 < |a_i x b_j| < 1e-6 (skipped by
+ * the guard), incident-face vertices that lie exactly on a clip line (kept by `da <= 0`), contacts the pair emitted */
+#define BBX_MAX 64
+#define BBX_W 9
 typedef struct {
   Model* m;
   /* state */
@@ -109,6 +115,9 @@ typedef struct {
   int* efc_type;
   int solver_iter, con_overflow, solver; /* solver: 0 = Newton (MuJoCo default, what the MJCF implies), 1 = PGS */
   int ncand;                             /* pairs that passed the broad phase in the last collision stage */
+  int nfound, ncon_peak;                 /* contacts the last collision stage found (uncapped); the most since orc_ncon_peak reset it */
+  int nbbx;                              /* box-box pairs the last collision stage ran col_box_box on (orc_field "boxbox") */
+  double bbx[BBX_MAX * BBX_W];
   double *tmp1, *tmp2, *nt_H, *nt_grad, *nt_search, *nt_Ma, *nt_Mv, *nt_jar, *nt_jv;
   int* nt_active;
 } Env;
@@ -418,6 +427,7 @@ static void make_frame(double* fr) { /* fr[0..2] = unit normal given; fill two t
 }
 static void add_contact(Env* e, int pair, double dist, const double* pos, const double* normal) {
   const Model* m = e->m;
+  if (++e->nfound > e->ncon_peak) e->ncon_peak = e->nfound;
   if (e->ncon >= e->maxcon) { e->con_overflow = 1; return; }
   Contact* c = &e->con[e->ncon++];
   c->dist = dist; v3copy(c->pos, pos); v3copy(c->frame, normal); make_frame(c->frame);
@@ -640,12 +650,13 @@ static void col_sphere_box(Env* e, int pair, int g1, int g2) {
 /* box-box: 15-axis SAT, then reference-face clipping (Sutherland-Hodgman) or edge-edge closest points.
  * DECISION: MuJoCo's mjc_BoxBox is not restated (undocumented); this is an independent manifold generator
  * with the same contract (<= 8 points, normal from geom1 to geom2, dist < margin). */
-static int clip_poly(double (*p)[2], int n, int axis, double lim, double (*out)[2]) {
+static int clip_poly(double (*p)[2], int n, int axis, double lim, double (*out)[2], double* on_line) {
   /* keep the part with sign*coord[axis] <= lim; called for +/- */
   int k = 0;
   for (int i = 0; i < n; i++) {
     const double *a = p[i], *b = p[(i + 1) % n];
     double da = a[axis] - lim, db = b[axis] - lim;
+    if (da == 0) *on_line += 1;
     if (da <= 0) { out[k][0] = a[0]; out[k][1] = a[1]; k++; }
     if ((da < 0 && db > 0) || (da > 0 && db < 0)) { double t = da / (da - db); out[k][0] = a[0] + t * (b[0] - a[0]); out[k][1] = a[1] + t * (b[1] - a[1]); k++; }
   }
@@ -657,26 +668,33 @@ static void col_box_box(Env* e, int pair, int g1, int g2) {
   const double *h1 = m->geom_size + 3 * g1, *h2 = m->geom_size + 3 * g2;
   double margin = m->pair_margin[pair];
   double d[3], a[3][3], b[3][3], C[3][3], AC[3][3];
+  double dummy[BBX_W], *rec = e->nbbx < BBX_MAX ? e->bbx + BBX_W * e->nbbx++ : dummy;
+  memset(rec, 0, sizeof(dummy));
+  rec[0] = g1; rec[1] = g2;
+  int ncon0 = e->ncon;
   v3sub(d, c2, c1);
   for (int i = 0; i < 3; i++) { m3col(a[i], R1, i); m3col(b[i], R2, i); }
   for (int i = 0; i < 3; i++) for (int j = 0; j < 3; j++) { C[i][j] = v3dot(a[i], b[j]); AC[i][j] = fabs(C[i][j]); }
-  double best_s = -1e300; int best_axis = -1;
+  double best_s = -1e300, face_s[6]; int best_axis = -1;
   for (int i = 0; i < 3; i++) { /* face axes of box 1 */
     double s = fabs(v3dot(d, a[i])) - (h1[i] + h2[0] * AC[i][0] + h2[1] * AC[i][1] + h2[2] * AC[i][2]);
     if (s >= margin) return;
     if (s > best_s) { best_s = s; best_axis = i; }
+    face_s[i] = s;
   }
   for (int j = 0; j < 3; j++) { /* face axes of box 2 */
     double s = fabs(v3dot(d, b[j])) - (h2[j] + h1[0] * AC[0][j] + h1[1] * AC[1][j] + h1[2] * AC[2][j]);
     if (s >= margin) return;
     if (s > best_s) { best_s = s; best_axis = 3 + j; }
+    face_s[3 + j] = s;
   }
+  for (int k = 0; k < 6; k++) rec[5] += face_s[k] == best_s;
   double edge_s = -1e300; int ei = -1, ej = -1; double en[3] = {0, 0, 0};
   for (int i = 0; i < 3; i++) for (int j = 0; j < 3; j++) {
     double L[3];
     v3cross(L, a[i], b[j]);
     double len = v3norm(L);
-    if (len < 1e-6) continue;
+    if (len < 1e-6) { rec[6] += len > 0; continue; }
     v3scl(L, L, 1.0 / len);
     double ra = 0, rb = 0;
     for (int k = 0; k < 3; k++) { ra += h1[k] * fabs(v3dot(L, a[k])); rb += h2[k] * fabs(v3dot(L, b[k])); }
@@ -705,10 +723,12 @@ static void col_box_box(Env* e, int pair, int g1, int g2) {
     if (dist >= margin) return;
     v3add(pos, q1, q2); v3scl(pos, pos, 0.5);
     add_contact(e, pair, dist, pos, n);
+    rec[2] = 2; rec[8] = e->ncon - ncon0;
     return;
   }
   /* face contact: reference box owns the axis */
   int ref1 = best_axis < 3, ax = ref1 ? best_axis : best_axis - 3;
+  rec[2] = 1; rec[3] = ref1 ? 1 : 2; rec[4] = best_axis;
   const double *cr = ref1 ? c1 : c2, *ci = ref1 ? c2 : c1, *hr = ref1 ? h1 : h2, *hi = ref1 ? h2 : h1;
   double (*ar)[3] = ref1 ? a : b;
   double (*ai)[3] = ref1 ? b : a;
@@ -743,13 +763,13 @@ static void col_box_box(Env* e, int pair, int g1, int g2) {
   double g0 = height[0] - gx * poly[0][0] - gy * poly[0][1];
   int n = 4;
   /* clip against the four side planes of the reference face */
-  n = clip_poly(poly, n, 0, hr[r1], tmp); if (!n) return;
+  n = clip_poly(poly, n, 0, hr[r1], tmp, rec + 7); if (!n) return;
   for (int k = 0; k < n; k++) { tmp[k][0] = -tmp[k][0]; }
-  n = clip_poly(tmp, n, 0, hr[r1], poly); if (!n) return;
+  n = clip_poly(tmp, n, 0, hr[r1], poly, rec + 7); if (!n) return;
   for (int k = 0; k < n; k++) { poly[k][0] = -poly[k][0]; }
-  n = clip_poly(poly, n, 1, hr[r2], tmp); if (!n) return;
+  n = clip_poly(poly, n, 1, hr[r2], tmp, rec + 7); if (!n) return;
   for (int k = 0; k < n; k++) { tmp[k][1] = -tmp[k][1]; }
-  n = clip_poly(tmp, n, 1, hr[r2], poly); if (!n) return;
+  n = clip_poly(tmp, n, 1, hr[r2], poly, rec + 7); if (!n) return;
   for (int k = 0; k < n; k++) { poly[k][1] = -poly[k][1]; }
   double n12[3];
   v3scl(n12, nref, ref1 ? 1.0 : -1.0);
@@ -763,6 +783,7 @@ static void col_box_box(Env* e, int pair, int g1, int g2) {
     add_contact(e, pair, dist, pos, n12);
     cnt++;
   }
+  rec[8] = e->ncon - ncon0;
 }
 
 /* ---- generic convex pair: Minkowski Portal Refinement (restates the published XenoCollide/MPR algorithm that MuJoCo
@@ -897,7 +918,7 @@ static int pair_is_analytic(int t1, int t2) {
  * (Contact order only affects floating-point summation order in the solver; the CUDA engine emits the same order.) */
 static void collision(Env* e) {
   const Model* m = e->m;
-  e->ncon = 0; e->con_overflow = 0; e->ncand = 0;
+  e->ncon = 0; e->con_overflow = 0; e->ncand = 0; e->nbbx = 0; e->nfound = 0;
   for (int pass = 0; pass < 2; pass++)
   for (int p = 0; p < m->npair; p++) {
     int g1 = m->pair_geom[2 * p], g2 = m->pair_geom[2 * p + 1], t1 = m->geom_type[g1], t2 = m->geom_type[g2];
@@ -1709,6 +1730,8 @@ int orc_sr_overflow(Env* e) { return e->sr_overflow; }
 void orc_efc_split(Env* e, int* out) { out[0] = e->ne; out[1] = e->nl; out[2] = e->nefc - e->ne - e->nl; }
 /* 1 if the last collision stage found more contacts than the capacity */
 int orc_con_overflow(Env* e) { return e->con_overflow; }
+/* the most contacts one collision stage found (capacity or not) since the previous call with reset != 0 */
+int orc_ncon_peak(Env* e, int reset) { int p = e->ncon_peak; if (reset) e->ncon_peak = 0; return p; }
 /* broad-phase survivors of the last collision stage (the engine's "ncand") */
 int orc_ncand(Env* e) { return e->ncand; }
 /* set_state + controller re-sync as GraspEnv.reset_model does (GraspingEnv.py:466-470) */
@@ -1733,7 +1756,7 @@ const double* orc_field(Env* e, const char* name, int* n) {
   F("qfrc_smooth", e->qfrc_smooth, m->nv) F("qacc_smooth", e->qacc_smooth, m->nv) F("qacc", e->qacc, m->nv)
   F("qfrc_constraint", e->qfrc_constraint, m->nv) F("efc_force", e->efc_force, e->nefc) F("efc_aref", e->efc_aref, e->nefc)
   F("efc_R", e->efc_R, e->nefc) F("efc_J", e->efc_J, e->nefc * m->nv) F("efc_pos", e->efc_pos, e->nefc)
-  F("gpos", e->gpos, 3 * m->ngeom) F("gmat", e->gmat, 9 * m->ngeom)
+  F("gpos", e->gpos, 3 * m->ngeom) F("gmat", e->gmat, 9 * m->ngeom) F("boxbox", e->bbx, BBX_W * e->nbbx)
 #undef F
   if (n) *n = 0;
   return NULL;

@@ -49,6 +49,7 @@ def lib():
         L.orc_sr_overflow.argtypes = [P]
         L.orc_efc_split.argtypes = [P, I]
         L.orc_ncand.argtypes = [P]
+        L.orc_ncon_peak.argtypes = [P, C.c_int]
         L.orc_reset.argtypes = [P, D, D]
         L.orc_field.restype = D
         L.orc_field.argtypes = [P, C.c_char_p, I]
@@ -176,6 +177,17 @@ class OracleEnv:
     def ncand(self):
         """pairs that passed the broad phase in the last collision stage"""
         return int(self.L.orc_ncand(self.env))
+
+    def ncon_peak(self, reset=True):
+        """the most contacts one collision stage found since the previous call with reset=True, counting those beyond the capacity"""
+        return int(self.L.orc_ncon_peak(self.env, 1 if reset else 0))
+
+    def boxbox(self):
+        """one row per box-box pair the last collision stage tested (col_box_box): geom1, geom2, outcome (0 separated, 1 face contact,
+        2 edge-edge), reference box (1 or 2, 0 unless a face contact), best face axis (0-2 box 1, 3-5 box 2), face axes whose
+        separation ties the best bit for bit, edge axes skipped by the 1e-6 guard with a non-zero cross product, incident vertices
+        exactly on a clip line, contacts emitted; int array [n, 9]"""
+        return self.field("boxbox").reshape(-1, 9).astype(np.int64)
 
     def forward(self):
         self.L.orc_forward(self.env)

@@ -29,10 +29,11 @@ def test_blob_roundtrip_and_sizes(scene_a):
 def test_compiler_reproduces_committed_blob():
     from mujoco_rl_ur5_b200.model.scene import compile_scene, load_scene
 
-    A, _ = load_scene("A")
-    M = compile_scene("A")
-    for k in ("body_mass", "body_inertia", "dof_invweight0", "pair_geom", "mesh_vert", "geom_obbhalf"):
-        assert np.allclose(np.asarray(M[k]).reshape(A[k].shape), A[k], rtol=1e-12, atol=1e-14), k
+    for key in ("A", "A1"):  # A1: the 6-object scene with its objects turned into 4 cm cubes (BASELINE config 3)
+        A, _ = load_scene(key)
+        M = compile_scene(key)
+        for k in ("body_mass", "body_inertia", "dof_invweight0", "pair_geom", "mesh_vert", "geom_obbhalf", "geom_size", "geom_type"):
+            assert np.allclose(np.asarray(M[k]).reshape(A[k].shape), A[k], rtol=1e-12, atol=1e-14), (key, k)
 
 
 def test_cabi_library_exports_every_declared_symbol():

@@ -91,6 +91,13 @@ int gq_sample_actions(const float* depth, const int* greedy_idx, const double* e
                       unsigned char* is_random, unsigned char* exhausted, void* stream);
 /* output.view(-1).max(0) per image (Grasping_Agent_multidiscrete.py:295-299): q [B,n] -> idx [B] int32 (rot*HW + y*W + x), val [B] f32 */
 int gq_argmax(const float* q, int B, int n, int* idx, float* val, void* stream);
+/* The Bellman target of the bootstrapped learn() (Grasping_Agent_multidiscrete.py:430-437: q_expected = reward + GAMMA *
+ * target_net(next_state).max(1)[0]) from the target network's head input, without the Q-map: x [B,H,W,64] bf16, w [A][64] f32,
+ * bias [A] f32 (A <= 8) as for gq_head_up2, reward [B] f32.  Out: qmax [B] f32 = the largest of the [A,2H,2W] sigmoids of each image,
+ * bit for bit the val of gq_argmax on the q of gq_head_up2; y [B] f32 = min(1, reward + gamma * qmax), product and sum each rounded to
+ * fp32 (no FMA), so that y stays in binary_cross_entropy's [0, 1] and equals reward at gamma = 0.  Deterministic. */
+int gq_head_max_target(const void* x, const float* w, const float* bias, const float* reward, float gamma, float* qmax, float* y, int B, int H, int W,
+                       int A, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------------------------------
  * Learner: the compute of Grasp_Agent.learn() (Grasping_Agent_multidiscrete.py:388-446, optimiser :153-156) - see csrc/qnet_learn.cuh.

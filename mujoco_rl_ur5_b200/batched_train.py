@@ -20,6 +20,14 @@ PrioritizedObservationReplay, every update draws its batch in proportion to the 
 trains on the importance-weighted loss with beta going linearly from beta0 to 1 over beta_updates updates, and writes the batch's new
 priorities (|r - q_pred| + eps)^alpha back.  Without it the trainer is the reference's uniform rule, unchanged.
 
+Bootstrapped Q-learning (`gamma` > 0, the reference's GAMMA branch of learn(), :105-115,140-144,410-413,430-437; default gamma = 0, the
+branch the reference runs): the replay also keeps each transition's next observation, keyed on the next batched step (key + N_total),
+so that its regenerated state is bit for bit the state the env acts on next; an episode's last transition bootstraps from the
+observation before the reset, as the reference does.  Before learner update u the target network (the learner's eval-mode,
+BatchNorm-folded forward) is rebuilt when u % target_update == 0 and after a construction or resume, and every update trains on
+y = min(1, r + gamma * max_a' Q_target(s', a')) (fp32; gq_head_max_target), which keeps y in binary_cross_entropy's [0, 1] (a successful
+grasp ends the bootstrapped return) and is r at gamma = 0.  With prioritized replay the priorities are |y - q_pred|.
+
 Multi-GPU (torchrun): rank r runs envs [r N, (r + 1) N) of N_total = world N, the learner all-reduces its gradients over the process
 group, each rank keeps its own replay and sampling stream random.Random(seed + rank), the counters are summed when a checkpoint is
 written and rank 0 writes it.
@@ -49,6 +57,20 @@ def per_beta(update, beta0, beta_updates):
     return beta0 + (1.0 - beta0) * min(1.0, update / beta_updates)
 
 
+def check_bootstrap(gamma, target_update):
+    """-> (gamma as a float, target_update); ValueError unless 0 <= gamma <= 1 and target_update is a positive int when gamma > 0 and
+    None when gamma = 0 (there is no target network then)"""
+    if isinstance(gamma, bool) or not isinstance(gamma, (int, float)) or not 0.0 <= float(gamma) <= 1.0:
+        raise ValueError(f"gamma must be a number in [0, 1], not {gamma!r}")
+    gamma = float(gamma)
+    if gamma > 0.0:
+        if isinstance(target_update, bool) or not isinstance(target_update, int) or target_update < 1:
+            raise ValueError(f"gamma > 0 needs target_update, a positive int (learner updates between target network syncs), not {target_update!r}")
+    elif target_update is not None:
+        raise ValueError(f"target_update is for gamma > 0 (there is no target network at gamma = 0); got {target_update!r}")
+    return gamma, target_update
+
+
 def epsilon(n, eps_start=EPS_START, eps_end=EPS_END, eps_decay=EPS_DECAY):
     """the reference's exploration rate of transition n (epsilon_greedy, :244-246), with its arithmetic (math.exp of -1.0 n / decay)"""
     return eps_end + (eps_start - eps_end) * math.exp(-1.0 * n / eps_decay)
@@ -65,10 +87,11 @@ def load_checkpoint(path_or_dict):
 class BatchedTrainer:
     def __init__(self, n_envs, scene="A", device=0, seed=0, batch_size=12, mem_size=None, updates_per_step=None, lr=1e-3, eps_start=EPS_START,
                  eps_end=EPS_END, eps_decay=EPS_DECAY, load=None, env_index_offset=None, n_total=None, process_group=None, chunk=64, max_draws=256,
-                 noise_std=0.001, log=None, prioritized=None):
+                 noise_std=0.001, log=None, prioritized=None, gamma=0.0, target_update=None):
         import torch
         import torch.distributed as dist
 
+        self.gamma, self.target_update = check_bootstrap(gamma, target_update)
         self.torch = torch
         self.pg = process_group
         rank, world = (dist.get_rank(process_group), dist.get_world_size(process_group)) if process_group is not None else (0, 1)
@@ -99,14 +122,15 @@ class BatchedTrainer:
         mem = max(2000, 4 * self.n_envs) if mem_size is None else int(mem_size)
         W, H = self.env.IMAGE_WIDTH, self.env.IMAGE_HEIGHT
         self.per = None
+        nxt = {"next_obs": True} if self.gamma > 0 else {}  # at gamma = 0 the replays are built exactly as without bootstrapping
         if prioritized is None:
-            self.replay = ObservationReplay(mem, (H, W), device=self.dev, rng=random.Random(self.seed + rank))
+            self.replay = ObservationReplay(mem, (H, W), device=self.dev, rng=random.Random(self.seed + rank), **nxt)
         else:
             unknown = set(prioritized) - set(PER_DEFAULTS) - {"beta_updates"}
             if unknown or "beta_updates" not in prioritized:
                 raise ValueError(f"prioritized takes alpha, beta0, beta_updates (required) and eps; got {sorted(prioritized)}")
             self.per = {**PER_DEFAULTS, **prioritized}
-            self.replay = PrioritizedObservationReplay(mem, (H, W), device=self.dev, alpha=self.per["alpha"], eps=self.per["eps"])
+            self.replay = PrioritizedObservationReplay(mem, (H, W), device=self.dev, alpha=self.per["alpha"], eps=self.per["eps"], **nxt)
         A = self.env.arrays
         cam = self.env.cam
         self.camera = (float(np.asarray(A["cam_fovy"]).ravel()[cam]), np.asarray(A["cam_pos0"], dtype=np.float64).reshape(-1, 3)[cam],
@@ -162,21 +186,21 @@ class BatchedTrainer:
         mark("start")
         _, act, rnd, exh = self.act(obs)
         mark("act")
-        _, reward, _, _ = env.step(act)
+        next_obs, reward, _, _ = env.step(act)
         mark("env_step")
         HW = env.IMAGE_WIDTH * env.IMAGE_HEIGHT
         flat = act[:, 1].to(t.int64) * HW + act[:, 0].to(t.int64)
+        nxt = {}
+        if self.gamma > 0:  # the next observation under the key the next batched step acts with
+            nxt = dict(next_rgb=next_obs["rgb"], next_depth=next_obs["depth"],
+                       next_steps=t.full((self.n_envs,), (self.steps_done + self.n_total) & 0xFFFFFFFF, dtype=t.int64))
         self.replay.push_batch(obs["rgb"], obs["depth"], flat, t.from_numpy(reward.astype(np.float32)), self.genv,
-                               t.full((self.n_envs,), key, dtype=t.int64))
+                               t.full((self.n_envs,), key, dtype=t.int64), **nxt)
         mark("push")
         losses = []
         if len(self.replay) >= 2 * self.batch_size:  # :396-399
             for _ in range(self.updates_per_step):
-                if self.per is None:
-                    s, a, r = self.replay.sample(self.batch_size, self.learner.fw, self.seed, self.depth_threshold, self.noise_std)
-                    losses.append(self.learner.learn_step(s, a, r))
-                else:
-                    losses.append(self.prioritized_update())
+                losses.append(self.update())
         mark("learn")
         # update_tensorboard's counters (:448-466), keyed by str(rotation) like the reference's defaultdicts
         rot = act[:, 1].cpu().numpy()
@@ -199,15 +223,38 @@ class BatchedTrainer:
             self.log.flush()
         return rec
 
+    def update(self):
+        """one learner update (the reference's learn()) on a batch drawn from the replay -> its loss"""
+        if self.per is not None:
+            return self.prioritized_update()
+        if self.gamma > 0:
+            s, a, r, s2 = self.replay.sample(self.batch_size, self.learner.fw, self.seed, self.depth_threshold, self.noise_std)
+            return self.learner.learn_step(s, a, self.bellman_targets(s2, r))
+        s, a, r = self.replay.sample(self.batch_size, self.learner.fw, self.seed, self.depth_threshold, self.noise_std)
+        return self.learner.learn_step(s, a, r)
+
     def prioritized_update(self):
         """one learner update on a prioritized batch: draw (keyed on the learner's update count and this rank), weighted learn step,
         new priorities of the drawn slots.  -> the weighted loss"""
         u = self.learner.step_count
         beta = per_beta(u, self.per["beta0"], self.per["beta_updates"])
-        s, a, r, idx, w = self.replay.sample(self.batch_size, self.learner.fw, self.seed, beta, u, self.rank, self.depth_threshold, self.noise_std)
+        out = self.replay.sample(self.batch_size, self.learner.fw, self.seed, beta, u, self.rank, self.depth_threshold, self.noise_std)
+        if self.gamma > 0:
+            s, a, r, s2, idx, w = out
+            r = self.bellman_targets(s2, r)
+        else:
+            s, a, r, idx, w = out
         loss, qsel = self.learner.learn_step(s, a, r, return_pred=True, weight=w)
         self.replay.update_priorities(idx, qsel, r)
         return loss
+
+    def bellman_targets(self, next_states, reward):
+        """y [B] f32 = min(1, r + gamma max_a' Q_target(s', a')) for the coming learner update; first rebuilds the target network from
+        the learner when it has none yet (a fresh or resumed trainer) or the update count is a multiple of target_update"""
+        L = self.learner
+        if L.target is None or L.step_count % self.target_update == 0:
+            L.sync_target()
+        return L.target.max_target(next_states, reward, self.gamma)[1]
 
     def train(self, episodes, steps_per_episode):
         for _ in range(episodes):
@@ -271,7 +318,13 @@ def main(argv=None):
     p.add_argument("--prioritized", action="store_true", help="prioritized experience replay (proportional); beta reaches 1 after the number of updates this run plans")
     p.add_argument("--per-alpha", type=float, default=PER_DEFAULTS["alpha"], help="priority exponent (with --prioritized)")
     p.add_argument("--per-beta0", type=float, default=PER_DEFAULTS["beta0"], help="initial importance-sampling exponent (with --prioritized)")
+    p.add_argument("--gamma", type=float, default=0.0, help="discount of the bootstrapped target r + gamma max Q_target(s') (0: the reward alone)")
+    p.add_argument("--target-update", type=int, default=None, help="learner updates between target network syncs (required with --gamma > 0)")
     a = p.parse_args(argv)
+    try:
+        check_bootstrap(a.gamma, a.target_update)
+    except ValueError as e:
+        p.error(str(e))
     import os
 
     import torch
@@ -289,7 +342,8 @@ def main(argv=None):
         per = dict(alpha=a.per_alpha, beta0=a.per_beta0, beta_updates=planned)
     tr = BatchedTrainer(a.envs, a.scene, device, seed=a.seed, batch_size=a.batch_size, mem_size=a.mem_size, updates_per_step=a.updates_per_step, lr=a.lr,
                         eps_start=a.eps_start, eps_end=a.eps_end, eps_decay=a.eps_decay, load=a.load, process_group=pg,
-                        log=sys.stdout if (pg is None or dist.get_rank() == 0) else None, prioritized=per)
+                        log=sys.stdout if (pg is None or dist.get_rank() == 0) else None, prioritized=per, gamma=a.gamma,
+                        target_update=a.target_update)
     try:
         tr.train(a.episodes, a.steps_per_episode)
         if a.out:

@@ -386,6 +386,41 @@ __global__ void k_upsample2x(const bf16* __restrict__ x, bf16* __restrict__ y, i
   }
   *(uint4*)(y + p * C + cv) = *(uint4*)o;
 }
+// The head's arithmetic, shared by gq_head_up2 (k_head + k_up2_sigmoid) and gq_head_max_target (k_head_max): the maximum of the
+// target network must be one of the Q-values of the forward, bit for bit, so both paths evaluate the same expressions.
+// the pixel's 64 channels (8 x 16 bytes of bf16) as floats
+__device__ __forceinline__ void head_load_pixel(const bf16* __restrict__ px, float (&in)[64]) {
+  const uint4* src = (const uint4*)px;
+#pragma unroll
+  for (int c = 0; c < 8; c++) {
+    const uint4 qv = __ldg(src + c);
+    const __nv_bfloat162* pv = (const __nv_bfloat162*)&qv;
+#pragma unroll
+    for (int k = 0; k < 4; k++) { float2 v = __bfloat1622float2(pv[k]); in[8 * c + 2 * k] = v.x; in[8 * c + 2 * k + 1] = v.y; }
+  }
+}
+// output plane a of the 1x1 convolution at one pixel; sw = the weights [A][64] f32 in shared memory, the biases at sw[8 * 64 + a]
+__device__ __forceinline__ float head_dot(const float (&in)[64], const float* sw, int a) {
+  float acc = sw[8 * 64 + a];
+#pragma unroll
+  for (int c = 0; c < 16; c++) {
+    float4 wv = ((const float4*)sw)[a * 16 + c];
+    acc += in[4 * c] * wv.x; acc += in[4 * c + 1] * wv.y; acc += in[4 * c + 2] * wv.z; acc += in[4 * c + 3] * wv.w;
+  }
+  return acc;
+}
+// source taps of output row (or column) o of UpsamplingBilinear2d(2) (align_corners=True) from n rows: rows i0, i1, weight w of i1
+struct Up2Tap { int i0, i1; float w; };
+__device__ __forceinline__ Up2Tap up2_tap(int o, int n) {
+  const float f = o * (float)(n - 1) / (float)(2 * n - 1);
+  const int i0 = (int)f;
+  return {i0, min(i0 + 1, n - 1), f - i0};
+}
+// sigmoid of the bilinear blend of z at (y0, x0) a, (y0, x1) b, (y1, x0) c, (y1, x1) d
+__device__ __forceinline__ float up2_sigmoid(float a, float b, float c, float d, float wx, float wy) {
+  const float v = (a * (1 - wx) + b * wx) * (1 - wy) + (c * (1 - wx) + d * wx) * wy;
+  return 1.f / (1.f + __expf(-v));
+}
 // last layer: conv1x1 64 -> A (+bias) before the sigmoid; x [B,HW,64] bf16, w [A][64] f32 -> z [B,A,HW] f32 (NCHW like the reference
 // output).  gq_head_up2 runs it on the low-resolution map and k_up2_sigmoid finishes the layer.
 __global__ void k_head(const bf16* __restrict__ x, const float* __restrict__ w, const float* __restrict__ bias, float* __restrict__ z, int B, int HW, int A) {
@@ -397,23 +432,8 @@ __global__ void k_head(const bf16* __restrict__ x, const float* __restrict__ w, 
   if (p >= (size_t)B * HW) return;
   int b = p / HW, pix = p % HW;
   float in[64];
-  const uint4* src = (const uint4*)(x + p * 64);  // the pixel's 64 channels = 8 x 16 bytes
-#pragma unroll
-  for (int c = 0; c < 8; c++) {
-    const uint4 qv = __ldg(src + c);
-    const __nv_bfloat162* pv = (const __nv_bfloat162*)&qv;
-#pragma unroll
-    for (int k = 0; k < 4; k++) { float2 v = __bfloat1622float2(pv[k]); in[8 * c + 2 * k] = v.x; in[8 * c + 2 * k + 1] = v.y; }
-  }
-  for (int a = 0; a < A; a++) {
-    float acc = sw[8 * 64 + a];
-#pragma unroll
-    for (int c = 0; c < 16; c++) {
-      float4 wv = ((const float4*)sw)[a * 16 + c];
-      acc += in[4 * c] * wv.x; acc += in[4 * c + 1] * wv.y; acc += in[4 * c + 2] * wv.z; acc += in[4 * c + 3] * wv.w;
-    }
-    z[((size_t)b * A + a) * HW + pix] = acc;
-  }
+  head_load_pixel(x + p * 64, in);
+  for (int a = 0; a < A; a++) z[((size_t)b * A + a) * HW + pix] = head_dot(in, sw, a);
 }
 // q = sigmoid(UpsamplingBilinear2d(2)(z)) on A planes: z [B*A, H, W] f32 -> q [B*A, 2H, 2W] f32 (align_corners=True).
 // The network ends with UP2 -> C1 (1x1 conv + bias) -> sigmoid (Modules.py:250-251,281-283); a 1x1 convolution is linear per pixel and the
@@ -424,13 +444,61 @@ __global__ void k_up2_sigmoid(const float* __restrict__ z, float* __restrict__ q
   if (i >= n) return;
   const int ow = i % OW, oh = (i / OW) % OH;
   const size_t pl = i / ((size_t)OW * OH);
-  const float fy = oh * (float)(H - 1) / (float)(OH - 1), fx = ow * (float)(W - 1) / (float)(OW - 1);
-  const int y0 = (int)fy, x0 = (int)fx, y1 = min(y0 + 1, H - 1), x1 = min(x0 + 1, W - 1);
-  const float wy = fy - y0, wx = fx - x0;
+  const Up2Tap ty = up2_tap(oh, H), tx = up2_tap(ow, W);
   const float* zp = z + pl * H * W;
-  const float a = __ldg(zp + y0 * W + x0), b = __ldg(zp + y0 * W + x1), c = __ldg(zp + y1 * W + x0), d = __ldg(zp + y1 * W + x1);
-  const float v = (a * (1 - wx) + b * wx) * (1 - wy) + (c * (1 - wx) + d * wx) * wy;
-  q[i] = 1.f / (1.f + __expf(-v));
+  q[i] = up2_sigmoid(__ldg(zp + ty.i0 * W + tx.i0), __ldg(zp + ty.i0 * W + tx.i1), __ldg(zp + ty.i1 * W + tx.i0), __ldg(zp + ty.i1 * W + tx.i1), tx.w, ty.w);
+}
+// max over the Q-map of every image without writing it: CTA (tx, ty, b) evaluates the head on the low-resolution pixels that its
+// HM_T x HM_T tile of the up-sampled map reads (z in shared memory) and the tile's A x HM_T x HM_T sigmoids, and raises qmax[b] to their
+// maximum with atomicMax on the float bits (exact and order-free: Q-values are >= +0, where the unsigned order of the bits is the float
+// order).  The largest sigmoid is taken, not the sigmoid of the largest pre-activation: __expf makes no promise of monotonicity.
+// Rows spanned by a tile: the source row f(o) = o (n - 1) / (2n - 1) grows by less than (HM_T - 1) / 2 over the tile, so floor(f) by at
+// most HM_T / 2, and with the second tap the tile reads at most HM_T / 2 + 2 rows (columns alike).
+constexpr int HM_T = 32, HM_Z = HM_T / 2 + 2;
+__global__ void __launch_bounds__(256) k_head_max(const bf16* __restrict__ x, const float* __restrict__ w, const float* __restrict__ bias,
+                                                  unsigned* __restrict__ qmax_bits, int H, int W, int A) {
+  __shared__ __align__(16) float sw[8 * 64 + 8];
+  __shared__ float sz[8][HM_Z][HM_Z];
+  __shared__ float swarp[8];
+  const int b = blockIdx.z, OH = 2 * H, OW = 2 * W;
+  const int oy0 = blockIdx.y * HM_T, ox0 = blockIdx.x * HM_T;
+  const int th = min(HM_T, OH - oy0), tw = min(HM_T, OW - ox0);
+  const int zy0 = up2_tap(oy0, H).i0, zx0 = up2_tap(ox0, W).i0;
+  const int zh = up2_tap(oy0 + th - 1, H).i1 - zy0 + 1, zw = up2_tap(ox0 + tw - 1, W).i1 - zx0 + 1;
+  for (int i = threadIdx.x; i < A * 64; i += blockDim.x) sw[i] = w[i];
+  if (threadIdx.x < A) sw[8 * 64 + threadIdx.x] = bias[threadIdx.x];
+  __syncthreads();
+  for (int i = threadIdx.x; i < zh * zw; i += blockDim.x) {
+    const int ly = i / zw, lx = i % zw;
+    float in[64];
+    head_load_pixel(x + (((size_t)b * H + zy0 + ly) * W + zx0 + lx) * 64, in);
+    for (int a = 0; a < A; a++) sz[a][ly][lx] = head_dot(in, sw, a);
+  }
+  __syncthreads();
+  float m = 0.f;
+  for (int i = threadIdx.x; i < A * th * tw; i += blockDim.x) {
+    const int a = i / (th * tw), r = i % (th * tw);
+    const Up2Tap ty = up2_tap(oy0 + r / tw, H), tx = up2_tap(ox0 + r % tw, W);
+    const int y0 = ty.i0 - zy0, y1 = ty.i1 - zy0, x0 = tx.i0 - zx0, x1 = tx.i1 - zx0;
+    const float v = up2_sigmoid(sz[a][y0][x0], sz[a][y0][x1], sz[a][y1][x0], sz[a][y1][x1], tx.w, ty.w);
+    m = v > m ? v : m;
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) { const float v = __shfl_xor_sync(0xffffffffu, m, o); m = v > m ? v : m; }
+  if ((threadIdx.x & 31) == 0) swarp[threadIdx.x >> 5] = m;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    for (int k = 1; k < (int)(blockDim.x >> 5); k++) m = swarp[k] > m ? swarp[k] : m;
+    atomicMax(qmax_bits + b, __float_as_uint(m));
+  }
+}
+// the Bellman target y = min(1, r + gamma * qmax) in fp32, product and sum rounded separately (no contraction); NaN propagates like
+// torch.clamp
+__global__ void k_bellman_target(const float* __restrict__ qmax, const float* __restrict__ reward, float gamma, float* __restrict__ y, int B) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= B) return;
+  const float v = __fadd_rn(reward[b], __fmul_rn(gamma, qmax[b]));
+  y[b] = v > 1.f ? 1.f : v;
 }
 // flat arg-max over the A*HW Q-values of every image (Grasping_Agent_multidiscrete.py:295-299): idx = rot*HW + y*W + x
 __global__ void __launch_bounds__(1024) k_argmax(const float* __restrict__ q, int n, int* __restrict__ idx, float* __restrict__ val) {
@@ -925,6 +993,16 @@ extern "C" int gq_head_up2(const void* x, const float* w, const float* bias, flo
   k_head<<<(unsigned)(((size_t)B * H * W + 127) / 128), 128, 0, st>>>((const bf16*)x, w, bias, scratch_z, B, H * W, A);
   size_t n = (size_t)B * A * 4 * H * W;
   k_up2_sigmoid<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(scratch_z, q, B * A, H, W);
+  QCK(cudaGetLastError());
+  return 0;
+}
+extern "C" int gq_head_max_target(const void* x, const float* w, const float* bias, const float* reward, float gamma, float* qmax, float* y, int B, int H,
+                                  int W, int A, void* stream) {
+  if (A < 1 || A > 8 || B < 1 || H < 1 || W < 1 || B > 65535) { snprintf(q_err, sizeof q_err, "gq_head_max_target: bad argument"); return -1; }
+  cudaStream_t st = (cudaStream_t)stream;
+  QCK(cudaMemsetAsync(qmax, 0, (size_t)B * sizeof(float), st));  // +0.0f: below every sigmoid value
+  k_head_max<<<dim3((2 * W + HM_T - 1) / HM_T, (2 * H + HM_T - 1) / HM_T, B), 256, 0, st>>>((const bf16*)x, w, bias, (unsigned*)qmax, H, W, A);
+  k_bellman_target<<<(B + 127) / 128, 128, 0, st>>>(qmax, reward, gamma, y, B);
   QCK(cudaGetLastError());
   return 0;
 }

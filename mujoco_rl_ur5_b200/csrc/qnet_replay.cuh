@@ -74,9 +74,9 @@ __global__ void __launch_bounds__(PER_THREADS) k_per_sample(const double* __rest
   if (j < B) w_out[j] = (float)(w / wmax);
 }
 
-// Priorities of a trained batch: p_j = (|r_j - q_j| + eps)^alpha (gamma = 0: the TD error is r - q_pred).  Leaves are written in
-// batch order - of a slot drawn more than once only the last entry writes - and then every entry walks its ancestors, one level per
-// barrier (entries sharing a node write the same sum).  pmax := max(pmax, max_j p_j).
+// Priorities of a trained batch: p_j = (|r_j - q_j| + eps)^alpha, r_j the training target (the reward at gamma = 0, the Bellman target
+// y with bootstrapping), so |r_j - q_j| is the TD error.  Leaves are written in batch order - of a slot drawn more than once only the
+// last entry writes - and then every entry walks its ancestors, one level per barrier (entries sharing a node write the same sum).  pmax := max(pmax, max_j p_j).
 __global__ void __launch_bounds__(PER_THREADS) k_per_update(double* __restrict__ tree, double* __restrict__ pmax, const long long* __restrict__ idx,
                                                             const float* __restrict__ qsel, const float* __restrict__ reward, int B, double alpha, double eps,
                                                             long long cap, int levels) {

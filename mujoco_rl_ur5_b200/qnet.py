@@ -24,7 +24,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 QLIB_PATH = os.path.join(_HERE, "csrc", "libgrasp_qnet.so")
 _QLIB = None
 QSYMBOLS = ["gq_last_error", "gq_version", "gq_conv_partials_floats", "gq_conv_tc", "gq_conv_tc_block_out", "gq_conv_first", "gq_maxpool", "gq_bn_act", "gq_upsample2x", "gq_head_up2", "gq_argmax", "gq_obs_to_state", "gq_obs_to_state_train", "gq_conv_tc_fused",
-            "gq_obs_to_state_keyed", "gq_sample_actions"]
+            "gq_obs_to_state_keyed", "gq_sample_actions", "gq_head_max_target"]
 
 
 def load_qnet_library():
@@ -47,6 +47,7 @@ def load_qnet_library():
         L.gq_upsample2x.argtypes = [P, P, I, I, I, I, P]
         L.gq_head_up2.argtypes = [P, P, P, P, P, I, I, I, I, P]
         L.gq_argmax.argtypes = [P, I, I, P, P, P]
+        L.gq_head_max_target.argtypes = [P, P, P, P, F, P, P, I, I, I, I, P]
         L.gq_obs_to_state.argtypes = [P, P, F, P, P, I, I, P]
         L.gq_obs_to_state_train.argtypes = [P, P, F, F, C.c_uint64, P, C.c_uint32, P, P, P, P, P, I, I, P]
         L.gq_obs_to_state_keyed.argtypes = [P, P, P, P, P, F, F, C.c_uint64, P, P, P, P, P, I, I, P]
@@ -239,7 +240,8 @@ class QNetForward:
         self._ck(self.L.gq_upsample2x(self._p(x), self._p(y), B, H, W, Cc, self._stream()), "gq_upsample2x")
         return y
 
-    def _forward_chunk(self, state):
+    def _trunk(self, state):
+        """every layer up to the head: state [B,4,H,W] f32 -> (x [B,H/2,W/2,64] bf16, the input of UP2 and C1, its height, its width)"""
         t = self.torch
         B, _, H, W = state.shape
         x = t.empty((B, H, W, 64), dtype=t.bfloat16, device=self.dev)
@@ -255,11 +257,20 @@ class QNetForward:
         x = self.basic_block(x, self.blocks[4], B, h2, w2)          # 1.RB2 256->128
         x = self.upsample(x.view(B, h2, w2, 128), B, h2, w2, 128)   # -> 100
         x = self.basic_block(x, self.blocks[5], B, 2 * h2, 2 * w2)  # 1.RB3 128->64
-        q = t.empty((B, self.A, 4 * h2, 4 * w2), dtype=t.float32, device=self.dev)
-        z = t.empty((B, self.A, 2 * h2, 2 * w2), dtype=t.float32, device=self.dev)
-        self._ck(self.L.gq_head_up2(self._p(x), self._p(self.w_head), self._p(self.b_head), self._p(z), self._p(q), B, 2 * h2, 2 * w2, self.A, self._stream()),
+        return x, 2 * h2, 2 * w2
+
+    def _head(self, x, h, w):
+        """UP2 -> C1 -> sigmoid on the head input x [B,h,w,64] bf16 -> Q [B,A,2h,2w] f32"""
+        t = self.torch
+        B = x.shape[0]
+        q = t.empty((B, self.A, 2 * h, 2 * w), dtype=t.float32, device=self.dev)
+        z = t.empty((B, self.A, h, w), dtype=t.float32, device=self.dev)
+        self._ck(self.L.gq_head_up2(self._p(x), self._p(self.w_head), self._p(self.b_head), self._p(z), self._p(q), B, h, w, self.A, self._stream()),
                  "gq_head_up2")
         return q
+
+    def _forward_chunk(self, state):
+        return self._head(*self._trunk(state))
 
     def forward(self, state):
         """state [B,4,H,W] f32 on the device -> Q [B,A,H,W] f32 (sigmoid), chunked to bound activation memory"""
@@ -267,6 +278,23 @@ class QNetForward:
         state = state.to(self.dev, t.float32).contiguous()
         outs = [self._forward_chunk(state[i:i + self.max_batch]) for i in range(0, state.shape[0], self.max_batch)]
         return outs[0] if len(outs) == 1 else t.cat(outs, dim=0)
+
+    def max_target(self, state, reward, gamma):
+        """the bootstrapped target of learn() (Grasping_Agent_multidiscrete.py:430-437) with this network as the target network:
+        state [B,4,H,W] f32 (the next states), reward [B] -> (qmax [B] f32 = Q(state).view(B, -1).max(1)[0], y [B] f32 =
+        min(1, reward + gamma * qmax) with gamma rounded to f32 and the product and the sum rounded separately).  Chunked like
+        `forward`; the Q-maps are never written (gq_head_max_target)."""
+        t = self.torch
+        state = state.to(self.dev, t.float32).contiguous()
+        B = state.shape[0]
+        reward = t.as_tensor(reward).to(self.dev, t.float32).reshape(B).contiguous()
+        qmax = t.empty(B, dtype=t.float32, device=self.dev)
+        y = t.empty(B, dtype=t.float32, device=self.dev)
+        for i in range(0, B, self.max_batch):
+            x, h, w = self._trunk(state[i:i + self.max_batch])
+            self._ck(self.L.gq_head_max_target(self._p(x), self._p(self.w_head), self._p(self.b_head), self._p(reward[i:]), float(gamma), self._p(qmax[i:]),
+                                               self._p(y[i:]), x.shape[0], h, w, self.A, self._stream()), "gq_head_max_target")
+        return qmax, y
 
     def obs_to_state(self, obs, depth_threshold=1.1):
         """batched deterministic transform_observation: obs dict of device tensors (rgb u8 [B,H,W,3], depth f32 [B,H,W]) -> [B,4,H,W] f32.

@@ -157,6 +157,7 @@ class QNetLearner:
         self.step_count = 0
         self.pg = process_group
         self.fw = None
+        self.target, self.target_step = None, None  # sync_target()
         self.launches = 0
         self._repack()
 
@@ -165,23 +166,30 @@ class QNetLearner:
         """fp32 parameters under the reference's names (parameters only; `model_state_dict()` adds the BatchNorm buffers)"""
         return {k: v.detach().clone() for k, v in self.p.items()}
 
-    def model_state_dict(self):
-        """the full state_dict of Modules.MULTIDISCRETE_RESNET(6): 51 parameters and 36 BatchNorm buffers, CPU fp32 (num_batches_tracked
-        int64), in the module's key order - loads with strict=True into the reference's network"""
-        t = self.torch
+    def device_state_dict(self):
+        """the 51 parameters and 24 BatchNorm running statistics as fp32 tensors on the learner's device, copied device to device, under
+        the reference's names (without num_batches_tracked, a host counter): what the eval-mode forward and the target network are
+        built from, with no host copy"""
         out = {}
         for k in model_keys():
             bn, _, leaf = k.rpartition(".")
             if k in self.p:
-                out[k] = self.p[k].detach().cpu().clone()
+                out[k] = self.p[k].detach().clone()
             elif leaf == "running_mean":
-                out[k] = self.running_mean[bn].detach().cpu().clone()
+                out[k] = self.running_mean[bn].detach().clone()
             elif leaf == "running_var":
-                out[k] = self.running_var[bn].detach().cpu().clone()
-            elif leaf == "num_batches_tracked":
-                out[k] = t.tensor(self.num_batches_tracked[bn], dtype=t.int64)
-            else:
-                raise KeyError(k)
+                out[k] = self.running_var[bn].detach().clone()
+        return out
+
+    def model_state_dict(self):
+        """the full state_dict of Modules.MULTIDISCRETE_RESNET(6): 51 parameters and 36 BatchNorm buffers, CPU fp32 (num_batches_tracked
+        int64), in the module's key order - loads with strict=True into the reference's network"""
+        t = self.torch
+        dev = self.device_state_dict()
+        out = {}
+        for k in model_keys():
+            bn, _, leaf = k.rpartition(".")
+            out[k] = t.tensor(self.num_batches_tracked[bn], dtype=t.int64) if leaf == "num_batches_tracked" else dev[k].cpu()
         return out
 
     def checkpoint(self):
@@ -213,7 +221,16 @@ class QNetLearner:
 
     def eval_forward(self, max_batch=64):
         """QNetForward in eval mode (batchnorm="running", BatchNorm folded into the weights) from the current parameters and buffers"""
-        return QNetForward(self.model_state_dict(), self.dev.index or 0, max_batch=max_batch, batchnorm="running")
+        return QNetForward(self.device_state_dict(), self.dev.index or 0, max_batch=max_batch, batchnorm="running")
+
+    def sync_target(self, max_batch=64):
+        """target network := the eval-mode forward of the current parameters and running statistics (the reference's
+        target_net.load_state_dict(policy_net.state_dict()) with target_net.eval(), Grasping_Agent_multidiscrete.py:105-115,410-413).
+        It is a separate copy: the learner's later steps do not change it.  Sets `target` and `target_step` (the step_count it was
+        built at); neither is part of a checkpoint."""
+        self.target = self.eval_forward(max_batch)
+        self.target_step = self.step_count
+        return self.target
 
     def _repack(self):
         """bf16 kernel layouts from the fp32 masters: the forward's [Cout][kh][kw][Cin] (QNetForward) and, for the input-gradient

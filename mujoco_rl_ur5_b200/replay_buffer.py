@@ -98,9 +98,13 @@ class ObservationReplay(_Ring):
     env int64, step int32 holding the uint32 key) against 640 012 B for the f32 state - and
     regenerates the training state at sample time with gq_obs_to_state_keyed.  That transform is a function of the observation and
     its key only, so a sampled state equals, bit for bit, the state the agent acted on when it pushed the transition.  Ring and
-    sampling are DeviceReplayBuffer's (the reference's B - 1 uniform picks plus the newest, from `rng`)."""
+    sampling are DeviceReplayBuffer's (the reference's B - 1 uniform picks plus the newest, from `rng`).
 
-    def __init__(self, size, image_hw=(200, 200), device="cuda", rng=None, seed=20):
+    next_obs=True (bootstrapped learning, the reference's `next_state`, Grasping_Agent_multidiscrete.py:140-144,551-554): each
+    transition also keeps the observation after its step and that observation's step key (280 004 B more at 200x200: rgb, depth,
+    uint32 key; the env is the transition's), and `sample` also returns the regenerated next states.  Off, nothing of it is stored."""
+
+    def __init__(self, size, image_hw=(200, 200), device="cuda", rng=None, seed=20, next_obs=False):
         super().__init__(size, device, rng, seed)
         t = self.torch
         H, W = image_hw
@@ -110,11 +114,25 @@ class ObservationReplay(_Ring):
         self.rewards = t.zeros(self.size, dtype=t.float32, device=self.device)
         self.envs = t.zeros(self.size, dtype=t.int64, device=self.device)
         self.steps = t.zeros(self.size, dtype=t.int32, device=self.device)  # the uint32 step key, bit for bit
+        self.next_obs = bool(next_obs)
+        self.next_rgb = self.next_depth = self.next_steps = None
+        if self.next_obs:
+            self.next_rgb = t.zeros_like(self.rgb)
+            self.next_depth = t.zeros_like(self.depth)
+            self.next_steps = t.zeros_like(self.steps)
 
-    def push_batch(self, rgb, depth, actions, rewards, envs, steps):
-        """N transitions in env order: observations [N,H,W,3] / [N,H,W], flat actions, rewards, global env ids and the step key"""
+    def _key32(self, steps):
+        """step keys (any integers) -> the int32 tensor holding their uint32 bit patterns"""
+        t = self.torch
+        return t.as_tensor(steps).to(t.int64).bitwise_and(0xFFFFFFFF).to(t.int32)
+
+    def push_batch(self, rgb, depth, actions, rewards, envs, steps, next_rgb=None, next_depth=None, next_steps=None):
+        """N transitions in env order: observations [N,H,W,3] / [N,H,W], flat actions, rewards, global env ids and the step key; with
+        next_obs the observations after the step (next_rgb, next_depth) and their step key (next_steps) too"""
         t = self.torch
         n = int(depth.shape[0])
+        if self.next_obs and (next_rgb is None or next_depth is None or next_steps is None):
+            raise ValueError("this replay stores next observations: push_batch needs next_rgb, next_depth and next_steps")
         skip, idx = self._claim(n)
         as_dev = lambda x, dt: t.as_tensor(x).to(self.device, dt).reshape(n)[skip:]
         self.rgb.index_copy_(0, idx, rgb[skip:].to(self.device))
@@ -122,16 +140,26 @@ class ObservationReplay(_Ring):
         self.actions.index_copy_(0, idx, as_dev(actions, t.int64))
         self.rewards.index_copy_(0, idx, as_dev(rewards, t.float32))
         self.envs.index_copy_(0, idx, as_dev(envs, t.int64))
-        self.steps.index_copy_(0, idx, as_dev(t.as_tensor(steps).to(t.int64).bitwise_and(0xFFFFFFFF).to(t.int32), t.int32))
+        self.steps.index_copy_(0, idx, as_dev(self._key32(steps), t.int32))
+        if self.next_obs:
+            self.next_rgb.index_copy_(0, idx, next_rgb[skip:].to(self.device))
+            self.next_depth.index_copy_(0, idx, next_depth[skip:].to(self.device, t.float32))
+            self.next_steps.index_copy_(0, idx, as_dev(self._key32(next_steps), t.int32))
+
+    def _states(self, idx, fwd, seed, depth_threshold, noise_std, nxt=False):
+        """the keyed training transform of the stored (nxt: next) observations of slots idx"""
+        rgb, depth, steps = (self.next_rgb, self.next_depth, self.next_steps) if nxt else (self.rgb, self.depth, self.steps)
+        return fwd.obs_to_state_keyed(rgb, depth, self.envs.index_select(0, idx), steps.index_select(0, idx), seed, slot=idx, depth_threshold=depth_threshold,
+                                      noise_std=noise_std)
 
     def sample(self, batch_size, fwd, seed, depth_threshold=1.1, noise_std=0.001):
-        """-> (states [B,4,H,W] f32, actions [B,1] int64, rewards [B,1] f32) in the reference's order; the states are regenerated by
-        `fwd` (a QNetForward on this buffer's device) with the keyed transform under `seed`"""
+        """-> (states [B,4,H,W] f32, actions [B,1] int64, rewards [B,1] f32) in the reference's order, with next_obs followed by the
+        next states [B,4,H,W] f32; the states are regenerated by `fwd` (a QNetForward on this buffer's device) with the keyed
+        transform under `seed`"""
         t = self.torch
         idx = t.as_tensor(self.sample_indices(batch_size), dtype=t.int64, device=self.device)
-        states = fwd.obs_to_state_keyed(self.rgb, self.depth, self.envs.index_select(0, idx), self.steps.index_select(0, idx), seed, slot=idx,
-                                        depth_threshold=depth_threshold, noise_std=noise_std)
-        return states, self.actions.index_select(0, idx)[:, None], self.rewards.index_select(0, idx)[:, None]
+        out = (self._states(idx, fwd, seed, depth_threshold, noise_std), self.actions.index_select(0, idx)[:, None], self.rewards.index_select(0, idx)[:, None])
+        return out + (self._states(idx, fwd, seed, depth_threshold, noise_std, nxt=True),) if self.next_obs else out
 
 
 class PrioritizedObservationReplay(ObservationReplay):
@@ -142,8 +170,8 @@ class PrioritizedObservationReplay(ObservationReplay):
     stratified (one uniform per 1/B of the total) and keyed on (seed, learner update, rank), so it needs no host generator and no
     host-to-device copy.  Priorities are not part of a checkpoint, like the stored transitions themselves."""
 
-    def __init__(self, size, image_hw=(200, 200), device="cuda", alpha=0.6, eps=1e-6):
-        super().__init__(size, image_hw, device, rng=None, seed=None)  # the uniform generator is not used (and the global one not re-seeded)
+    def __init__(self, size, image_hw=(200, 200), device="cuda", alpha=0.6, eps=1e-6, next_obs=False):
+        super().__init__(size, image_hw, device, rng=None, seed=None, next_obs=next_obs)  # the uniform generator is not used (nor the global one re-seeded)
         from .qnet import load_qnet_library
         from .qnet_learn import _bind_learn
 
@@ -169,9 +197,9 @@ class PrioritizedObservationReplay(ObservationReplay):
         self._claimed = idx
         return skip, idx
 
-    def push_batch(self, rgb, depth, actions, rewards, envs, steps):
+    def push_batch(self, rgb, depth, actions, rewards, envs, steps, next_rgb=None, next_depth=None, next_steps=None):
         """ObservationReplay.push_batch, then the claimed slots' priorities := pmax (gq_per_push)"""
-        super().push_batch(rgb, depth, actions, rewards, envs, steps)
+        super().push_batch(rgb, depth, actions, rewards, envs, steps, next_rgb, next_depth, next_steps)
         slots = self._claimed.contiguous()
         self._ck(self.L.gq_per_push(self.tree.data_ptr(), self.pmax.data_ptr(), slots.data_ptr(), int(slots.numel()), self.cap, self._st()), "gq_per_push")
 
@@ -187,16 +215,19 @@ class PrioritizedObservationReplay(ObservationReplay):
         return idx, w
 
     def sample(self, batch_size, fwd, seed, beta, update, rank=0, depth_threshold=1.1, noise_std=0.001):
-        """-> (states [B,4,H,W] f32, actions [B,1] int64, rewards [B,1] f32, idx [B] int64, weights [B] f32); the draw is keyed on
-        (seed, update, rank) - the trainer passes the learner's update count and its process rank - and the states are regenerated
-        by `fwd` (a QNetForward on this buffer's device) with the keyed transform under `seed`"""
+        """-> (states [B,4,H,W] f32, actions [B,1] int64, rewards [B,1] f32, idx [B] int64, weights [B] f32), with next_obs the next
+        states [B,4,H,W] f32 after the rewards; the draw is keyed on (seed, update, rank) - the trainer passes the learner's update
+        count and its process rank - and the states are regenerated by `fwd` (a QNetForward on this buffer's device) with the keyed
+        transform under `seed`"""
         idx, w = self.sample_slots(batch_size, beta, seed, update, rank)
-        states = fwd.obs_to_state_keyed(self.rgb, self.depth, self.envs.index_select(0, idx), self.steps.index_select(0, idx), seed, slot=idx,
-                                        depth_threshold=depth_threshold, noise_std=noise_std)
-        return states, self.actions.index_select(0, idx)[:, None], self.rewards.index_select(0, idx)[:, None], idx, w
+        out = (self._states(idx, fwd, seed, depth_threshold, noise_std), self.actions.index_select(0, idx)[:, None], self.rewards.index_select(0, idx)[:, None])
+        if self.next_obs:
+            out += (self._states(idx, fwd, seed, depth_threshold, noise_std, nxt=True),)
+        return out + (idx, w)
 
     def update_priorities(self, idx, qsel, reward):
-        """priorities of the slots idx [B] after training on them: (|reward - qsel| + eps)^alpha, in batch order (gq_per_update)"""
+        """priorities of the slots idx [B] after training on them: (|reward - qsel| + eps)^alpha, in batch order (gq_per_update); `reward`
+        is the training target, the Bellman target y when the trainer bootstraps"""
         t = self.torch
         idx = idx.to(self.device, t.int64).reshape(-1).contiguous()
         B = int(idx.numel())

@@ -144,6 +144,12 @@ int gq_upsample2x_bwd(const void* dY, void* dX, int B, int H, int W, int C, void
 int gq_add_to_bf16(const float* a, const float* b, const void* c_bf16, void* out, size_t n, void* stream);
 /* torch.optim.Adam step with weight_decay as L2 (Grasping_Agent_multidiscrete.py:153-156): p, g, m, v [n] f32, step counted from 1 */
 int gq_adam(float* p, const float* g, float* m, float* v, size_t n, float lr, float beta1, float beta2, float eps, float weight_decay, int step, void* stream);
+/* torch.optim.SGD step with dampening 0 and nesterov off (Grasping_Agent_multidiscrete.py:145-152, momentum 0.9, weight_decay 2e-5):
+ * d = g + wd p; buf = d when `first` (the buffer's first step), else momentum buf + d; p -= lr buf.  p, g, buf [n] f32; with momentum 0
+ * there is no buffer (buf may be NULL) and p -= lr d.  Each product and sum is rounded separately (no FMA contraction). */
+int gq_sgd(float* p, const float* g, float* buf, size_t n, float lr, float momentum, float weight_decay, int first, void* stream);
+/* gradient accumulation over micro-batches: acc = g when `first`, else acc + g (fp32, [n]) */
+int gq_grad_accumulate(float* acc, const float* g, size_t n, int first, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------------------------------
  * Prioritized experience replay (Schaul et al. 2016, proportional) - see csrc/qnet_replay.cuh.  tree [2 cap] f64: an implicit sum-tree,

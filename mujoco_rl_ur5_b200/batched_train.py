@@ -28,6 +28,13 @@ BatchNorm-folded forward) is rebuilt when u % target_update == 0 and after a con
 y = min(1, r + gamma * max_a' Q_target(s', a')) (fp32; gq_head_max_target), which keeps y in binary_cross_entropy's [0, 1] (a successful
 grasp ends the bootstrapped return) and is r at gamma = 0.  With prioritized replay the priorities are |y - q_pred|.
 
+Optimiser and accumulation (`optimizer`, `momentum`, `accumulate`; the reference's OPTIMIZER and NUMBER_ACCUMULATIONS_BEFORE_UPDATE):
+Adam by default, or SGD with momentum; a loaded checkpoint brings its own.  With accumulate = K one update draws batch_size * K
+transitions in one call (the reference's BATCH_SIZE = MAX_POSSIBLE_SAMPLES * K; with prioritized replay K * batch_size strata whose
+importance weights are normalised over the whole draw), QNetLearner.learn_step trains on them as K micro-batches of batch_size with one
+optimizer step, and updating starts once the replay holds 2 * batch_size * K transitions.  At gamma > 0 the targets of all the drawn
+next states come from the one target network before the step.  `updates` in the per-step record counts optimizer steps.
+
 Multi-GPU (torchrun): rank r runs envs [r N, (r + 1) N) of N_total = world N, the learner all-reduces its gradients over the process
 group, each rank keeps its own replay and sampling stream random.Random(seed + rank), the counters are summed when a checkpoint is
 written and rank 0 writes it.
@@ -42,7 +49,7 @@ from collections import defaultdict
 import numpy as np
 
 from .batched_env import BatchedGraspEnv
-from .qnet_learn import QNetLearner
+from .qnet_learn import QNetLearner, check_optimizer
 from .replay_buffer import ObservationReplay, PrioritizedObservationReplay
 
 EPS_START, EPS_END, EPS_DECAY = 1.0, 0.2, 8000   # Grasping_Agent_multidiscrete.py:35-37
@@ -87,11 +94,12 @@ def load_checkpoint(path_or_dict):
 class BatchedTrainer:
     def __init__(self, n_envs, scene="A", device=0, seed=0, batch_size=12, mem_size=None, updates_per_step=None, lr=1e-3, eps_start=EPS_START,
                  eps_end=EPS_END, eps_decay=EPS_DECAY, load=None, env_index_offset=None, n_total=None, process_group=None, chunk=64, max_draws=256,
-                 noise_std=0.001, log=None, prioritized=None, gamma=0.0, target_update=None):
+                 noise_std=0.001, log=None, prioritized=None, gamma=0.0, target_update=None, optimizer=None, momentum=0.9, accumulate=1):
         import torch
         import torch.distributed as dist
 
         self.gamma, self.target_update = check_bootstrap(gamma, target_update)
+        _, self.accumulate, momentum = check_optimizer("adam" if optimizer is None else optimizer, accumulate, momentum)
         self.torch = torch
         self.pg = process_group
         rank, world = (dist.get_rank(process_group), dist.get_world_size(process_group)) if process_group is not None else (0, 1)
@@ -108,10 +116,13 @@ class BatchedTrainer:
         self.chunk, self.max_draws, self.noise_std = int(chunk), int(max_draws), float(noise_std)
         self.log = log
         ckpt = None if load is None else load_checkpoint(load)
+        opt = {} if optimizer is None else {"optimizer": optimizer}
         if ckpt is None:
-            self.learner = QNetLearner(None, device, lr=lr, seed=self.seed, process_group=process_group)
-        else:  # as the reference's constructor: the optimizer state (and with it the learning rate) comes from the checkpoint (:157-179)
-            self.learner = QNetLearner.from_checkpoint(ckpt, device, process_group=process_group)
+            self.learner = QNetLearner(None, device, lr=lr, seed=self.seed, process_group=process_group, momentum=momentum, accumulate=self.accumulate,
+                                       **opt)
+        else:  # as the reference's constructor: the optimizer state (and with it the optimizer, learning rate and momentum) comes from the
+            # checkpoint (:157-179); an explicit optimizer must be the checkpoint's
+            self.learner = QNetLearner.from_checkpoint(ckpt, device, process_group=process_group, accumulate=self.accumulate, **opt)
         ckpt = ckpt or {}
         self.steps_done = int(ckpt.get("step", 0))
         # as the reference (:161-163, :182): EPS_START for a fresh agent, the checkpoint's value or EPS_STEADY = 0 for a loaded one
@@ -198,7 +209,7 @@ class BatchedTrainer:
                                t.full((self.n_envs,), key, dtype=t.int64), **nxt)
         mark("push")
         losses = []
-        if len(self.replay) >= 2 * self.batch_size:  # :396-399
+        if len(self.replay) >= 2 * self.batch_size * self.accumulate:  # :396-399, BATCH_SIZE = MAX_POSSIBLE_SAMPLES * accumulations
             for _ in range(self.updates_per_step):
                 losses.append(self.update())
         mark("learn")
@@ -224,13 +235,15 @@ class BatchedTrainer:
         return rec
 
     def update(self):
-        """one learner update (the reference's learn()) on a batch drawn from the replay -> its loss"""
+        """one learner update (the reference's learn()) on a batch of batch_size * accumulate transitions drawn from the replay in one
+        call -> its loss"""
         if self.per is not None:
             return self.prioritized_update()
+        n = self.batch_size * self.accumulate
         if self.gamma > 0:
-            s, a, r, s2 = self.replay.sample(self.batch_size, self.learner.fw, self.seed, self.depth_threshold, self.noise_std)
+            s, a, r, s2 = self.replay.sample(n, self.learner.fw, self.seed, self.depth_threshold, self.noise_std)
             return self.learner.learn_step(s, a, self.bellman_targets(s2, r))
-        s, a, r = self.replay.sample(self.batch_size, self.learner.fw, self.seed, self.depth_threshold, self.noise_std)
+        s, a, r = self.replay.sample(n, self.learner.fw, self.seed, self.depth_threshold, self.noise_std)
         return self.learner.learn_step(s, a, r)
 
     def prioritized_update(self):
@@ -238,7 +251,7 @@ class BatchedTrainer:
         new priorities of the drawn slots.  -> the weighted loss"""
         u = self.learner.step_count
         beta = per_beta(u, self.per["beta0"], self.per["beta_updates"])
-        out = self.replay.sample(self.batch_size, self.learner.fw, self.seed, beta, u, self.rank, self.depth_threshold, self.noise_std)
+        out = self.replay.sample(self.batch_size * self.accumulate, self.learner.fw, self.seed, beta, u, self.rank, self.depth_threshold, self.noise_std)
         if self.gamma > 0:
             s, a, r, s2, idx, w = out
             r = self.bellman_targets(s2, r)
@@ -283,10 +296,11 @@ class BatchedTrainer:
         return out
 
     def checkpoint(self):
-        """the dict the reference's main() saves (:560-572)"""
+        """the dict the reference's main() saves (:560-572); with SGD also the learner's "learner_step" (QNetLearner.checkpoint)"""
         ck = self.learner.checkpoint()
+        extra = {"learner_step": ck["learner_step"]} if "learner_step" in ck else {}
         return {"step": self.steps_done, "model_state_dict": ck["model_state_dict"], "optimizer_state_dict": ck["optimizer_state_dict"],
-                "epsilon": self.eps_threshold, **self.counters()}
+                "epsilon": self.eps_threshold, **self.counters(), **extra}
 
     def save(self, path):
         """writes the checkpoint from rank 0 (every rank must call it: the counters are summed over the ranks)"""
@@ -306,7 +320,7 @@ def main(argv=None):
     p.add_argument("--episodes", type=int, default=1)
     p.add_argument("--steps-per-episode", type=int, default=50)
     p.add_argument("--updates-per-step", type=int, default=None, help="learn() calls per batched step (default: --envs, one per transition)")
-    p.add_argument("--batch-size", type=int, default=12)
+    p.add_argument("--batch-size", type=int, default=12, help="transitions per forward/backward (the reference's MAX_POSSIBLE_SAMPLES)")
     p.add_argument("--mem-size", type=int, default=None, help="replay capacity per GPU (default: max(2000, 4 envs))")
     p.add_argument("--lr", type=float, default=1e-3)
     p.add_argument("--eps-start", type=float, default=EPS_START)
@@ -320,9 +334,14 @@ def main(argv=None):
     p.add_argument("--per-beta0", type=float, default=PER_DEFAULTS["beta0"], help="initial importance-sampling exponent (with --prioritized)")
     p.add_argument("--gamma", type=float, default=0.0, help="discount of the bootstrapped target r + gamma max Q_target(s') (0: the reward alone)")
     p.add_argument("--target-update", type=int, default=None, help="learner updates between target network syncs (required with --gamma > 0)")
+    p.add_argument("--optimizer", choices=("adam", "sgd"), default=None, help="adam, or sgd with momentum (default: the --load checkpoint's, else adam)")
+    p.add_argument("--momentum", type=float, default=0.9, help="SGD momentum of a fresh run (a loaded checkpoint keeps its own)")
+    p.add_argument("--accumulate", type=int, default=1,
+                   help="micro-batches of --batch-size per optimizer step, gradients summed (the reference's NUMBER_ACCUMULATIONS_BEFORE_UPDATE)")
     a = p.parse_args(argv)
     try:
         check_bootstrap(a.gamma, a.target_update)
+        check_optimizer(a.optimizer or "adam", a.accumulate, a.momentum)
     except ValueError as e:
         p.error(str(e))
     import os
@@ -343,7 +362,7 @@ def main(argv=None):
     tr = BatchedTrainer(a.envs, a.scene, device, seed=a.seed, batch_size=a.batch_size, mem_size=a.mem_size, updates_per_step=a.updates_per_step, lr=a.lr,
                         eps_start=a.eps_start, eps_end=a.eps_end, eps_decay=a.eps_decay, load=a.load, process_group=pg,
                         log=sys.stdout if (pg is None or dist.get_rank() == 0) else None, prioritized=per, gamma=a.gamma,
-                        target_update=a.target_update)
+                        target_update=a.target_update, optimizer=a.optimizer, momentum=a.momentum, accumulate=a.accumulate)
     try:
         tr.train(a.episodes, a.steps_per_episode)
         if a.out:

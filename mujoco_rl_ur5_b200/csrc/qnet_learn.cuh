@@ -333,6 +333,31 @@ __global__ void k_adam(float* __restrict__ p, const float* __restrict__ g, float
   p[i] -= lr * (mm / bc1) / (sqrtf(vv / bc2) + eps);
 }
 
+// ------------------------------------------------------------------------------------------------ SGD (torch.optim.SGD, dampening 0, nesterov off)
+// p, g, buf fp32 [n]:  d = g + wd p;  buf = d (first step) or momentum buf + d;  p -= lr buf        (Grasping_Agent_multidiscrete.py:145-152:
+// lr, momentum 0.9, wd 2e-5).  momentum = 0: no buffer, p -= lr d.  Every product and sum is rounded on its own (__fmul_rn / __fadd_rn: no
+// contraction into an FMA), in torch's order - mul_(momentum) then add_(d); add_(buf, alpha=-lr).  Where torch's own kernels fuse
+// `a + alpha b` into one FMA, the result differs from it by at most half an ulp of wd p and of lr buf.
+__global__ void k_sgd(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ buf, size_t n, float lr, float momentum, float wd, int first) {
+  size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const float pp = p[i];
+  float d = __fadd_rn(g[i], __fmul_rn(wd, pp));
+  if (buf) {
+    d = first ? d : __fadd_rn(__fmul_rn(momentum, buf[i]), d);
+    buf[i] = d;
+  }
+  p[i] = __fsub_rn(pp, __fmul_rn(lr, d));
+}
+
+// ------------------------------------------------------------------------------------------------ gradient accumulation over micro-batches
+// acc = g (first micro-batch) or acc + g, fp32 [n]: torch's .grad accumulation of successive backward() calls, micro-batch 1 first
+__global__ void k_grad_accumulate(float* __restrict__ acc, const float* __restrict__ g, size_t n, int first) {
+  size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  acc[i] = first ? g[i] : __fadd_rn(acc[i], g[i]);
+}
+
 // ------------------------------------------------------------------------------------------------ C-ABI
 extern "C" int gq_bn_batch_merge(float* stats, int B, int C, void* stream) {
   if (!stats || B <= 0 || C <= 0) { snprintf(q_err, sizeof q_err, "gq_bn_batch_merge: bad argument"); return -1; }
@@ -567,6 +592,20 @@ extern "C" int gq_adam(float* p, const float* g, float* m, float* v, size_t n, f
   if (!p || !g || !m || !v || step < 1) { snprintf(q_err, sizeof q_err, "gq_adam: bad argument"); return -1; }
   const float bc1 = 1.f - powf(beta1, (float)step), bc2 = 1.f - powf(beta2, (float)step);
   k_adam<<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(p, g, m, v, n, lr, beta1, beta2, eps, weight_decay, bc1, bc2);
+  QCK(cudaGetLastError());
+  return 0;
+}
+extern "C" int gq_sgd(float* p, const float* g, float* buf, size_t n, float lr, float momentum, float weight_decay, int first, void* stream) {
+  if (!p || !g || (momentum != 0.f && !buf) || !(momentum >= 0.f)) { snprintf(q_err, sizeof q_err, "gq_sgd: bad argument"); return -1; }
+  if (n == 0) return 0;
+  k_sgd<<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(p, g, momentum != 0.f ? buf : nullptr, n, lr, momentum, weight_decay, first);
+  QCK(cudaGetLastError());
+  return 0;
+}
+extern "C" int gq_grad_accumulate(float* acc, const float* g, size_t n, int first, void* stream) {
+  if (!acc || !g) { snprintf(q_err, sizeof q_err, "gq_grad_accumulate: bad argument"); return -1; }
+  if (n == 0) return 0;
+  k_grad_accumulate<<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(acc, g, n, first);
   QCK(cudaGetLastError());
   return 0;
 }

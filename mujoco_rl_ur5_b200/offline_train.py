@@ -30,7 +30,7 @@ import numpy as np
 
 from . import offline_data
 from .qnet import make_torch_qnet
-from .qnet_learn import QNetLearner
+from .qnet_learn import QNetLearner, check_optimizer
 
 DEPTH_THRESHOLD = 1.1  # grasping_dataset.py:45
 NOISE_STD = 0.001      # grasping_dataset.py:51
@@ -116,10 +116,15 @@ def rng_plan(n, epochs, batch_size=15, seed=30):
 
 
 class OfflineTrainer:
-    def __init__(self, data, device=0, batch_size=15, lr=1e-3, weight_decay=2e-5, epochs=20, seed=30, load=None):
+    def __init__(self, data, device=0, batch_size=15, lr=1e-3, weight_decay=2e-5, epochs=20, seed=30, load=None, optimizer=None, momentum=0.9):
         """data: path of a transition file (offline_data / the reference's generate_data, unite_data, extract_positives) or the tuple
-        offline_data.load_transitions returns; load: None, a checkpoint path or a {"model_state_dict", "optimizer_state_dict"} dict"""
+        offline_data.load_transitions returns; load: None, a checkpoint path or a {"model_state_dict", "optimizer_state_dict"} dict;
+        optimizer: "adam" or "sgd" (torch.optim.SGD with `momentum`); None is Adam for a fresh run and the checkpoint's optimiser
+        with `load`, which also brings its own lr, momentum and weight decay"""
         import torch
+
+        check_optimizer("adam" if optimizer is None else optimizer, 1, momentum)
+        opt = {} if optimizer is None else {"optimizer": optimizer}
 
         self.torch = torch
         self.dev = torch.device("cuda", device)
@@ -132,9 +137,9 @@ class OfflineTrainer:
         net, self.train_loader, self.test_loader = rng_setup(self.n, self.batch_size, self.seed)
         if load is not None:
             ckpt = load if isinstance(load, dict) else torch.load(load, map_location="cpu", weights_only=False)
-            self.learner = QNetLearner.from_checkpoint(ckpt, device)  # lr / weight decay from the checkpoint, as optimizer.load_state_dict does (:86)
+            self.learner = QNetLearner.from_checkpoint(ckpt, device, **opt)  # lr / weight decay from the checkpoint, as optimizer.load_state_dict does (:86)
         else:
-            self.learner = QNetLearner(net.state_dict(), device, lr=lr, weight_decay=weight_decay)
+            self.learner = QNetLearner(net.state_dict(), device, lr=lr, weight_decay=weight_decay, momentum=momentum, **opt)
         del net
         self.rgb = torch.as_tensor(np.ascontiguousarray(rgb)).to(self.dev)
         self.depth = torch.as_tensor(np.ascontiguousarray(depth, dtype=np.float32)).to(self.dev)
@@ -205,7 +210,8 @@ class OfflineTrainer:
         return self.learner.checkpoint()
 
     def save(self, path):
-        """writes {"model_state_dict", "optimizer_state_dict"} like train.py:147-163 (loads into Modules.MULTIDISCRETE_RESNET + Adam)"""
+        """writes {"model_state_dict", "optimizer_state_dict"} like train.py:147-163 (loads into Modules.MULTIDISCRETE_RESNET + Adam, or
+        SGD with "learner_step" added)"""
         self.torch.save(self.checkpoint(), path)
 
 
@@ -220,8 +226,14 @@ def main(argv=None):
     ap.add_argument("--device", type=int, default=0)
     ap.add_argument("--load", default=None, help="checkpoint to continue from ({'model_state_dict', 'optimizer_state_dict'})")
     ap.add_argument("--out", default=None, help="where to save the final checkpoint")
+    ap.add_argument("--optimizer", choices=("adam", "sgd"), default=None, help="adam, or sgd with momentum (default: the --load checkpoint's, else adam)")
+    ap.add_argument("--momentum", type=float, default=0.9, help="SGD momentum of a fresh run (a loaded checkpoint keeps its own)")
     a = ap.parse_args(argv)
-    tr = OfflineTrainer(a.data, a.device, a.batch_size, a.lr, a.weight_decay, a.epochs, a.seed, a.load)
+    try:
+        check_optimizer(a.optimizer or "adam", 1, a.momentum)
+    except ValueError as e:
+        ap.error(str(e))
+    tr = OfflineTrainer(a.data, a.device, a.batch_size, a.lr, a.weight_decay, a.epochs, a.seed, a.load, optimizer=a.optimizer, momentum=a.momentum)
     t0 = time.perf_counter()
     tr.run(log=print)
     dt = time.perf_counter() - t0

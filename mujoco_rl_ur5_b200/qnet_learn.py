@@ -17,9 +17,15 @@ training-mode forward does (momentum 0.1, unbiased variance; gq_bn_running_updat
 running statistics, from its own shard of the batch; write checkpoints from rank 0, which is what DDP's default broadcast_buffers
 amounts to.  The ranks' statistics are not synchronised.
 
+Optimiser: Adam (default) or, with optimizer="sgd", torch.optim.SGD(lr, momentum 0.9, weight_decay) - the reference's OPTIMIZER = "SGD"
+(:41,145-152), gq_sgd.  Gradient accumulation (accumulate = K, the reference's NUMBER_ACCUMULATIONS_BEFORE_UPDATE, :27-31,408-446): one
+learn_step takes K micro-batches, each with its own training-mode forward and a backward of loss / K; the gradients are summed in order
+(gq_grad_accumulate) and one optimizer step follows.  K = 1 with Adam is the single-batch step, kernel for kernel.
+
 Checkpoints in the reference's format (Offline RL/train.py:84-86,147-163, Grasping_Agent_multidiscrete.py:111-158,561-572):
 `checkpoint()` -> {"model_state_dict", "optimizer_state_dict"}, `QNetLearner.from_checkpoint(ckpt)` restores parameters, buffers and the
-Adam state (m, v, step).  The optimizer part is produced and read by a CPU torch.optim.Adam, so its format is torch's own.
+optimiser state (Adam: m, v, step; SGD: the momentum buffers, and the step count from the extra "learner_step" key).  The optimizer part is
+produced and read by a CPU torch.optim.Adam / torch.optim.SGD, so its format is torch's own.
 """
 import ctypes as C
 
@@ -91,6 +97,59 @@ def adam_from_torch(opt_state):
     return m, v, steps.pop(), hyper
 
 
+def sgd_to_torch(params, buf, lr, momentum, weight_decay):
+    """flat SGD state -> torch.optim.SGD(lr, momentum, dampening=0, weight_decay, nesterov=False).state_dict() over
+    make_torch_qnet(6).parameters().  params / buf: dicts name -> tensor (the reference's parameter names); buf None: no momentum buffer
+    yet (before the first step, or momentum = 0), which torch's SGD state then leaves empty"""
+    import torch
+
+    net = _cpu_qnet()
+    with torch.no_grad():
+        for k, p in net.named_parameters():
+            p.copy_(params[k].detach().cpu())
+    opt = torch.optim.SGD(net.parameters(), lr=lr, momentum=momentum, dampening=0, weight_decay=weight_decay, nesterov=False)
+    if buf is not None:
+        for k, p in net.named_parameters():
+            opt.state[p] = {"momentum_buffer": buf[k].detach().cpu().clone().to(torch.float32)}
+    return opt.state_dict()
+
+
+def sgd_from_torch(opt_state):
+    """torch.optim.SGD state_dict (over make_torch_qnet(6).parameters()) -> (buf, hyper): buf a dict name -> CPU tensor of the momentum
+    buffers, or None when the optimiser holds none (before its first step, or momentum = 0); hyper = dict(lr, momentum, weight_decay) of
+    its parameter group.  A parameter group without the keys newer torch versions added (maximize, foreach, differentiable, fused) loads
+    with their defaults.  Nesterov momentum, dampening and maximize are refused: the learner implements none of them."""
+    import torch
+
+    g = opt_state["param_groups"][0]
+    bad = {k: g.get(k, d) for k, d in (("nesterov", False), ("dampening", 0), ("maximize", False)) if g.get(k, d) != d}
+    if bad:
+        raise ValueError(f"the SGD state uses {bad}; the learner's SGD has nesterov=False, dampening=0 and maximize=False only")
+    net = _cpu_qnet()
+    with torch.no_grad():
+        for p in net.parameters():
+            p.zero_()
+    opt = torch.optim.SGD(net.parameters(), lr=1.0)
+    opt.load_state_dict(opt_state)
+    have = [opt.state.get(p, {}).get("momentum_buffer") for p in net.parameters()]
+    if any(b is None for b in have) and any(b is not None for b in have):
+        raise ValueError("the optimizer state has momentum buffers for some parameters only; the learner keeps one for all or none")
+    buf = None if have[0] is None else {k: b.detach().clone() for (k, _), b in zip(net.named_parameters(), have)}
+    g = opt.param_groups[0]
+    return buf, dict(lr=float(g["lr"]), momentum=float(g["momentum"]), weight_decay=float(g["weight_decay"]))
+
+
+def optimizer_of(opt_state):
+    """"adam" or "sgd": the optimiser a torch optimizer state_dict belongs to, told by its parameter group (Adam's has betas, SGD's
+    momentum and dampening)"""
+    g = opt_state["param_groups"][0]
+    if "betas" in g:
+        return "adam"
+    if "momentum" in g and "dampening" in g:
+        return "sgd"
+    raise ValueError(f"the optimizer state is neither Adam's nor SGD's (parameter group keys {sorted(g)})")
+
+
 def _bind_learn(L):
     P, I, F = C.c_void_p, C.c_int, C.c_float
     if getattr(L, "_learn_bound", False):
@@ -104,6 +163,8 @@ def _bind_learn(L):
     L.gq_upsample2x_bwd.argtypes = [P, P, I, I, I, I, P]
     L.gq_add_to_bf16.argtypes = [P, P, P, P, C.c_size_t, P]
     L.gq_adam.argtypes = [P, P, P, P, C.c_size_t, F, F, F, F, F, I, P]
+    L.gq_sgd.argtypes = [P, P, P, C.c_size_t, F, F, F, I, P]
+    L.gq_grad_accumulate.argtypes = [P, P, C.c_size_t, I, P]
     L.gq_bn_running_update.argtypes = [P, P, P, I, I, I, F, P]
     L.gq_loss_head_bwd_weighted.argtypes = [P, P, P, P, P, P, I, I, I, I, P, P, P, P, P, P, P, P]
     D, U64 = C.c_double, C.c_uint64
@@ -115,13 +176,32 @@ def _bind_learn(L):
 
 
 LEARN_SYMBOLS = ["gq_bn_batch_merge", "gq_loss_head_bwd", "gq_bn_relu_bwd", "gq_conv_wgrad", "gq_conv_first_wgrad", "gq_maxpool_bwd", "gq_upsample2x_bwd",
-                 "gq_add_to_bf16", "gq_adam", "gq_bn_running_update", "gq_loss_head_bwd_weighted", "gq_per_push", "gq_per_sample", "gq_per_update"]
+                 "gq_add_to_bf16", "gq_adam", "gq_bn_running_update", "gq_loss_head_bwd_weighted", "gq_per_push", "gq_per_sample", "gq_per_update",
+                 "gq_sgd", "gq_grad_accumulate"]
+OPTIMIZERS = ("adam", "sgd")
+
+
+def check_optimizer(optimizer, accumulate, momentum=0.9):
+    """-> (optimizer, accumulate, momentum as a float); ValueError unless optimizer is "adam" or "sgd", accumulate (micro-batches per
+    update) an int >= 1 and momentum a finite number >= 0"""
+    if optimizer not in OPTIMIZERS:
+        raise ValueError(f"optimizer must be one of {OPTIMIZERS}, not {optimizer!r}")
+    if isinstance(accumulate, bool) or not isinstance(accumulate, int) or accumulate < 1:
+        raise ValueError(f"accumulate (micro-batches per optimizer step) must be an int >= 1, not {accumulate!r}")
+    if isinstance(momentum, bool) or not isinstance(momentum, (int, float)) or not 0.0 <= float(momentum) < float("inf"):
+        raise ValueError(f"momentum must be a finite number >= 0, not {momentum!r}")
+    return optimizer, accumulate, float(momentum)
 
 
 class QNetLearner:
-    def __init__(self, state_dict=None, device=0, lr=0.001, weight_decay=0.00002, betas=(0.9, 0.999), eps=1e-8, seed=0, process_group=None):
+    def __init__(self, state_dict=None, device=0, lr=0.001, weight_decay=0.00002, betas=(0.9, 0.999), eps=1e-8, seed=0, process_group=None,
+                 optimizer="adam", momentum=0.9, accumulate=1):
+        """optimizer: "adam" (torch.optim.Adam(lr, betas, eps, weight_decay)) or "sgd" (torch.optim.SGD(lr, momentum, weight_decay), the
+        reference's OPTIMIZER = "SGD"); accumulate = K: every learn_step takes K micro-batches and makes one optimizer step on the sum
+        of their gradients, each loss scaled by 1 / K (the reference's NUMBER_ACCUMULATIONS_BEFORE_UPDATE)"""
         import torch
 
+        self.optimizer, self.accumulate, momentum = check_optimizer(optimizer, accumulate, momentum)
         if not torch.cuda.is_available():
             raise RuntimeError("QNetLearner needs a CUDA device (there is no CPU fallback)")
         self.torch = torch
@@ -137,8 +217,15 @@ class QNetLearner:
         n = int(self.offsets[-1])
         self.flat = torch.empty(n, dtype=torch.float32, device=self.dev)
         self.grad = torch.zeros(n, dtype=torch.float32, device=self.dev)
-        self.m = torch.zeros(n, dtype=torch.float32, device=self.dev)
-        self.v = torch.zeros(n, dtype=torch.float32, device=self.dev)
+        # optimiser state: Adam's moments, or SGD's momentum buffer (none at momentum 0) and whether its first step has set it
+        sgd = self.optimizer == "sgd"
+        self.m = None if sgd else torch.zeros(n, dtype=torch.float32, device=self.dev)
+        self.v = None if sgd else torch.zeros(n, dtype=torch.float32, device=self.dev)
+        self.momentum = momentum
+        self.momentum_buf = torch.zeros(n, dtype=torch.float32, device=self.dev) if sgd and self.momentum != 0.0 else None
+        self.momentum_init = False
+        # the sum of the micro-batches' gradients (accumulate > 1 only; with one micro-batch the optimiser reads `grad`)
+        self.grad_acc = torch.zeros(n, dtype=torch.float32, device=self.dev) if self.accumulate > 1 else None
         self.p, self.g = {}, {}
         for k, o, sz in zip(self.names, self.offsets[:-1], sizes):
             shape = tuple(state_dict[k].shape)
@@ -194,7 +281,13 @@ class QNetLearner:
 
     def checkpoint(self):
         """{"model_state_dict", "optimizer_state_dict"} as the reference saves them (Offline RL/train.py:147-163); the optimizer part is
-        torch.optim.Adam's own state_dict (step, exp_avg = m, exp_avg_sq = v; lr / betas / eps / weight_decay)"""
+        torch.optim.Adam's own state_dict (step, exp_avg = m, exp_avg_sq = v; lr / betas / eps / weight_decay) or, with optimizer="sgd",
+        torch.optim.SGD's (momentum_buffer; lr / momentum / dampening 0 / weight_decay / nesterov False).  torch's SGD state has no step
+        counter, so an SGD checkpoint also carries "learner_step" (step_count), which torch.load and the reference ignore."""
+        if self.optimizer == "sgd":
+            buf = self._flat_views(self.momentum_buf) if self.momentum_init else None
+            return {"model_state_dict": self.model_state_dict(), "optimizer_state_dict": sgd_to_torch(self.p, buf, self.lr, self.momentum, self.wd),
+                    "learner_step": int(self.step_count)}
         return {"model_state_dict": self.model_state_dict(),
                 "optimizer_state_dict": adam_to_torch(self.p, self._flat_views(self.m), self._flat_views(self.v), self.step_count, self.lr, self.betas,
                                                       self.eps, self.wd)}
@@ -202,11 +295,30 @@ class QNetLearner:
     @classmethod
     def from_checkpoint(cls, ckpt, device=0, **kw):
         """learner from a {"model_state_dict", "optimizer_state_dict"} checkpoint (written by `checkpoint()` or by the reference's scripts):
-        parameters, BatchNorm buffers, Adam moments and step count; lr / betas / eps / weight_decay from the optimizer's parameter group
-        unless given in `kw`.  A checkpoint without "optimizer_state_dict" starts a fresh optimiser."""
+        parameters, BatchNorm buffers and the optimiser's state.  The optimiser is the checkpoint's: Adam (its parameter group has betas;
+        moments and step count restored) or SGD (momentum; momentum buffers restored, step count from "learner_step").  An explicit
+        `optimizer=` in `kw` that disagrees is a ValueError.  lr / betas / eps / momentum / weight_decay come from the parameter group
+        unless given in `kw`.  A checkpoint without "optimizer_state_dict" starts a fresh optimiser.
+
+        The reference's own SGD checkpoints have no "learner_step": they resume at step_count 0, which restarts what counts learner
+        updates - prioritized replay's beta schedule (and its sampling keys) and the phase of the target network's sync period."""
         opt = ckpt.get("optimizer_state_dict")
         if opt is None:
             return cls(ckpt["model_state_dict"], device, **kw)
+        kind = optimizer_of(opt)
+        if kw.get("optimizer", kind) != kind:
+            raise ValueError(f"optimizer={kw['optimizer']!r} was asked for, but the checkpoint holds the state of {kind!r}")
+        kw = {**kw, "optimizer": kind}
+        if kind == "sgd":
+            buf, hyper = sgd_from_torch(opt)
+            L = cls(ckpt["model_state_dict"], device, **{**hyper, **kw})
+            if buf is not None and L.momentum_buf is not None:
+                bv = L._flat_views(L.momentum_buf)
+                for k in L.names:
+                    bv[k].copy_(buf[k].to(L.dev, L.torch.float32))
+                L.momentum_init = True
+            L.step_count = int(ckpt.get("learner_step", 0))
+            return L
         m, v, step, hyper = adam_from_torch(opt)
         L = cls(ckpt["model_state_dict"], device, **{**hyper, **kw})
         mv, vv = L._flat_views(L.m), L._flat_views(L.v)
@@ -363,11 +475,12 @@ class QNetLearner:
     # parameter groups in the order the backward pass completes them (each one contiguous in the flat buffers)
     GROUPS = ("1.C1.", "1.RB3.", "1.RB2.", "1.RB1.", "0.RB3.", "0.RB2.", "0.RB1.", "0.C1.")
 
-    def grad_slice(self, prefix):
-        """the contiguous piece of the flat gradient buffer that holds every parameter whose name starts with `prefix`"""
+    def grad_slice(self, prefix, flat=None):
+        """the contiguous piece of the flat gradient buffer (or of `flat`, laid out alike) that holds every parameter whose name starts
+        with `prefix`"""
         idx = [i for i, k in enumerate(self.names) if k.startswith(prefix)]
         assert idx and idx == list(range(idx[0], idx[-1] + 1)), prefix
-        return self.grad[int(self.offsets[idx[0]]):int(self.offsets[idx[-1] + 1])]
+        return (self.grad if flat is None else flat)[int(self.offsets[idx[0]]):int(self.offsets[idx[-1] + 1])]
 
     def backward(self, q, saved, action, reward, on_ready=None, weight=None):
         """-> loss (0-dim tensor), q_pred [B]; fills self.grad (every parameter gradient of the step).  `on_ready(prefix)` is called as
@@ -430,26 +543,72 @@ class QNetLearner:
         [B,1].  Returns the loss as a float (one device->host read, like the reference's `loss.item()`); with return_pred=True
         (loss, q_pred [B] on the device), q_pred being the gathered Q-values of the training forward (Offline RL/train.py:109,122).
         weight: None (the reference's loss) or [B] f32 importance weights on the device; the step then minimises and returns the
-        weighted loss binary_cross_entropy(q_pred, reward, weight=weight)."""
+        weighted loss binary_cross_entropy(q_pred, reward, weight=weight).
+
+        With accumulate = K the B rows (B divisible by K) are K micro-batches of B / K consecutive rows, as the reference's learn() slices
+        its BATCH_SIZE = K * MAX_POSSIBLE_SAMPLES draw: each one gets its own training-mode forward (its own BatchNorm statistics and one
+        running-statistics update) and a backward of its loss / K (weights w_b / K, w_b = 1 without importance weights), the gradients
+        are summed in micro-batch order (gq_grad_accumulate), then one optimizer step.  The loss returned is the sum of the scaled
+        losses, i.e. the mean of the micro-batch losses; q_pred holds all B gathered Q-values in row order."""
         t = self.torch
-        q, saved = self.forward_train(state)
-        works = []
-        on_ready = None
-        if self.pg is not None:
+        K = self.accumulate
+        B = int(state.shape[0])
+        if B % K:
+            raise ValueError(f"learn_step: {B} rows do not split into accumulate = {K} equal micro-batches")
+        if K == 1:  # (the arguments as given: no slicing on the single-batch path)
+            micro = [(state, action, reward, weight)]
+        else:
+            b = B // K
+            action, reward = action.reshape(B), reward.reshape(B)
+            wb = t.ones(B, dtype=t.float32, device=self.dev) if weight is None else weight.to(self.dev, t.float32).reshape(B)
+            weight = wb / K
+            micro = [(state[k * b:(k + 1) * b], action[k * b:(k + 1) * b], reward[k * b:(k + 1) * b], weight[k * b:(k + 1) * b]) for k in range(K)]
+        works, losses, qsels = [], [], []
+        for k, (s, a, r, w) in enumerate(micro):
+            q, saved = self.forward_train(s)
+            on_ready = None
+            if K > 1 or self.pg is not None:
+                on_ready = self._on_ready(works, first=k == 0, reduce=k == K - 1)
+            loss, qsel = self.backward(q, saved, a, r, on_ready, w)
+            losses.append(loss)
+            qsels.append(qsel)
+        for work in works:
+            work.wait()  # (stream-level wait: the optimizer step below is ordered after the last piece)
+        self.step_count += 1
+        self._optimizer_step(self.grad if K == 1 else self.grad_acc)
+        self._repack()
+        loss = losses[0] if K == 1 else t.stack(losses).sum()
+        qsel = qsels[0] if K == 1 else t.cat(qsels)
+        return (float(loss), qsel) if return_pred else float(loss)
+
+    def _on_ready(self, works, first, reduce):
+        """the per-parameter-group hook of one micro-batch's backward: with accumulate > 1 the group's gradient is added into grad_acc,
+        and on the last micro-batch (`reduce`) with a process group the group's summed gradient is averaged over the ranks"""
+        dist = None
+        if self.pg is not None and reduce:
             import torch.distributed as dist
 
-            # the learner's one collective: the 29.3 MB of fp32 gradients averaged over the ranks, issued per parameter group (8 pieces,
-            # last layers first) on NCCL's stream as soon as the group's last wgrad kernel is enqueued, so that the transfer of the
-            # 512/256-channel blocks runs under the backward pass of the layers in front of them (Grasping_Agent_multidiscrete.py has a
-            # single process; this is north_star's "gradient/batch reduction")
-            def on_ready(prefix):
-                works.append(dist.all_reduce(self.grad_slice(prefix), op=dist.ReduceOp.AVG, group=self.pg, async_op=True))
+        def on_ready(prefix):
+            g = self.grad_slice(prefix)
+            if self.accumulate > 1:
+                acc = self.grad_slice(prefix, self.grad_acc)
+                self._ck(self.L.gq_grad_accumulate(self._p(acc), self._p(g), g.numel(), int(first), self._st()), "gq_grad_accumulate")
+                g = acc
+            if dist is not None:
+                # the learner's one collective: the 29.3 MB of fp32 gradients averaged over the ranks, issued per parameter group (8 pieces,
+                # last layers first) on NCCL's stream as soon as the group's last wgrad kernel is enqueued, so that the transfer of the
+                # 512/256-channel blocks runs under the backward pass of the layers in front of them (Grasping_Agent_multidiscrete.py has a
+                # single process; this is north_star's "gradient/batch reduction").  With accumulation: once per optimizer step, the sum.
+                works.append(dist.all_reduce(g, op=dist.ReduceOp.AVG, group=self.pg, async_op=True))
 
-        loss, qsel = self.backward(q, saved, action, reward, on_ready, weight)
-        for w in works:
-            w.wait()  # (stream-level wait: Adam below is ordered after the last piece)
-        self.step_count += 1
-        self._ck(self.L.gq_adam(self._p(self.flat), self._p(self.grad), self._p(self.m), self._p(self.v), self.flat.numel(), self.lr, self.betas[0], self.betas[1],
-                                self.eps, self.wd, self.step_count, self._st()), "gq_adam")
-        self._repack()
-        return (float(loss), qsel) if return_pred else float(loss)
+        return on_ready
+
+    def _optimizer_step(self, grad):
+        """one step of the learner's optimiser on the flat gradient `grad` (step_count already counts it)"""
+        if self.optimizer == "adam":
+            self._ck(self.L.gq_adam(self._p(self.flat), self._p(grad), self._p(self.m), self._p(self.v), self.flat.numel(), self.lr, self.betas[0],
+                                    self.betas[1], self.eps, self.wd, self.step_count, self._st()), "gq_adam")
+            return
+        self._ck(self.L.gq_sgd(self._p(self.flat), self._p(grad), self._p(self.momentum_buf), self.flat.numel(), self.lr, self.momentum, self.wd,
+                               int(not self.momentum_init), self._st()), "gq_sgd")
+        self.momentum_init = self.momentum_buf is not None

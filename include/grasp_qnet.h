@@ -80,6 +80,23 @@ int gq_obs_to_state_train(const unsigned char* rgb, const float* depth, float de
 int gq_obs_to_state_keyed(const unsigned char* rgb, const float* depth, const long long* slot, const long long* env_index, const unsigned int* step,
                           float depth_threshold, float noise_std, unsigned long long seed, float* scratch_red, float* jitter_out, int* order_out,
                           float* state, void* state_nhwc_bf16, int B, int HW, void* stream);
+/* Grasp_Agent.transform_observation(normalize=False) batched (Grasping_Agent_multidiscrete.py:311-354, statistics read by get_mean_std
+ * :370-379): the observation standardised with normalize.py's channel statistics.  Row b of the output is image slot[b] of rgb [S,HW,3] u8 /
+ * depth [S,HW] f32 (slot [B] int64, NULL: b), keyed on env_index[b] (int64, NULL: b) and steps[b] (uint32, NULL: `step`) as in
+ * gq_obs_to_state_keyed.  mean_std: 8 host floats (mean r, g, b, depth, std r, g, b, depth), each std > 0.  Per pixel, every operation
+ * rounded on its own (no FMA): r' = (r - mean_r) / std_r with r in 0..255 (likewise g, b); d' = (min(d, depth_threshold) - mean_d) / std_d
+ * + noise_std * z, z = the standard normal of gq_obs_to_state_train's depth noise at (seed, env, step, pixel).  No ColorJitter.
+ * Outputs (either may be NULL): state [B,4,HW] f32, state_nhwc_bf16 [B,HW,4] bf16.  B < 1 or a std <= 0 returns -1 before any launch. */
+int gq_obs_to_state_standard(const unsigned char* rgb, const float* depth, const long long* slot, const long long* env_index, const unsigned int* steps,
+                             unsigned int step, const float* mean_std, float depth_threshold, float noise_std, unsigned long long seed, float* state,
+                             void* state_nhwc_bf16, int B, int HW, void* stream);
+/* normalize.py (:20-66) over B observations: out [8] f64 (device) = mean r, g, b, depth, std r, g, b, depth, population std (ddof 0) over
+ * all B*HW pixels; rgb [B,HW,3] u8, depth [B,HW] f32 metres (no threshold).  RGB from exact integer sums: the means are np.mean's bit for
+ * bit, the stds sqrt(n sum x^2 - (sum x)^2) / n with the 128-bit numerator rounded once.  Depth in fp64 (sum, then the sum of squared
+ * deviations from the fp64 mean), each result rounded to f32 once (stored exactly in out[3], out[7]).  Deterministic (fixed order, no
+ * atomics).  scratch: gq_obs_channel_stats_scratch_bytes(B*HW) bytes.  B*HW < 2^44. */
+size_t gq_obs_channel_stats_scratch_bytes(long long n_pixels);
+int gq_obs_channel_stats(const unsigned char* rgb, const float* depth, int B, int HW, void* scratch, double* out, void* stream);
 /* Grasp_Agent.epsilon_greedy (Grasping_Agent_multidiscrete.py:232-282) for B envs.  depth [B,H,W] f32 (the current observation),
  * greedy_idx [B] int32 (gq_argmax), eps [B] f64, env_index [B] int64 (global env ids), seed / step: key and counter of the keyed draws.
  * Env b is greedy iff its uniform u > eps[b]; otherwise it takes the first of its candidates (flat rot*H*W + y*W + x) whose pixel lies

@@ -5,6 +5,10 @@ flat arg-max -> transform_action (:381-386); `epsilon_greedy` (:232-282) mixes i
 Here: gq_obs_to_state -> wgmma Q-network forward -> gq_argmax, all kernels of libgrasp_qnet.so; the result is an int32
 [N,2] tensor (pixel index, rotation index) that BatchedGraspEnv.step accepts without leaving the GPU (BASELINE config 4).
 The learner (replay buffer, BCE loss, Adam; :388-446) is a SURVEY 8(f) "next" row and is not part of this class.
+
+standardize=<mean_and_std path or its 8 values> acts on transform_observation(normalize=False) instead (gq_obs_to_state_standard,
+obs_stats): channels standardised with normalize.py's statistics and the depth noise N(0, noise_std) in standardised units, which the
+reference adds on every such call; the noise is keyed on (seed, global env id, acting call), the call counted by `acting_step`.
 """
 import numpy as np
 
@@ -12,8 +16,17 @@ from .qnet import QNetForward, make_torch_qnet
 
 
 class BatchedGreedyAgent:
-    def __init__(self, env, state_dict=None, seed=0, chunk=64):
+    standardize = None  # the min-max transform unless __init__ is given statistics (also for agents assembled field by field)
+
+    def __init__(self, env, state_dict=None, seed=0, chunk=64, standardize=None, noise_std=0.001):
         import torch
+
+        from .batched_train import resolve_standardize
+
+        self.standardize = resolve_standardize(standardize)
+        self.noise_std = float(noise_std)
+        self.seed = int(seed)
+        self.acting_step = 0
 
         self.torch = torch
         self.env = env
@@ -27,8 +40,19 @@ class BatchedGreedyAgent:
         self.gen = torch.Generator(device=env.engine.device)
         self.gen.manual_seed(seed)
 
+    def states(self, obs):
+        """the state the agent acts on: the deterministic min-max transform, or with `standardize` the standardised one (each call
+        draws the next acting step's noise)"""
+        if self.standardize is None:
+            return self.qnet.obs_to_state(obs, self.depth_threshold)
+        t = self.torch
+        genv = self.env.env_index_offset + t.arange(obs["depth"].shape[0], dtype=t.int64, device=obs["depth"].device)
+        s = self.qnet.obs_to_state_standard(obs, self.standardize, self.depth_threshold, self.noise_std, self.seed, self.acting_step, genv)
+        self.acting_step += 1
+        return s
+
     def q_values(self, obs):
-        return self.qnet.forward(self.qnet.obs_to_state(obs, self.depth_threshold))
+        return self.qnet.forward(self.states(obs))
 
     def greedy(self, obs):
         """[N,2] int32 actions on the device and their Q-values"""

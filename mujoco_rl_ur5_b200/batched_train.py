@@ -35,6 +35,12 @@ importance weights are normalised over the whole draw), QNetLearner.learn_step t
 optimizer step, and updating starts once the replay holds 2 * batch_size * K transitions.  At gamma > 0 the targets of all the drawn
 next states come from the one target network before the step.  `updates` in the per-step record counts optimizer steps.
 
+Standardised observations (`standardize` = a `mean_and_std` path or its 8 values; the reference's transform_observation(normalize=False),
+:311-354): the acting states, the replay's regenerated states (next states at gamma > 0 included) and so the epsilon-greedy arg-max use
+gq_obs_to_state_standard under the same (seed, env, step) keys, with the depth noise noise_std in standardised units and no ColorJitter;
+gq_sample_actions still reads the raw depth.  The checkpoint gains "mean_and_std"; a resume from such a checkpoint uses its values, and
+passing different ones is an error.  Without it every state, the replay and the checkpoint are the min-max path's.
+
 Multi-GPU (torchrun): rank r runs envs [r N, (r + 1) N) of N_total = world N, the learner all-reduces its gradients over the process
 group, each rank keeps its own replay and sampling stream random.Random(seed + rank), the counters are summed when a checkpoint is
 written and rank 0 writes it.
@@ -83,6 +89,22 @@ def epsilon(n, eps_start=EPS_START, eps_end=EPS_END, eps_decay=EPS_DECAY):
     return eps_end + (eps_start - eps_end) * math.exp(-1.0 * n / eps_decay)
 
 
+def resolve_standardize(standardize, ckpt=None):
+    """-> the 8 statistics (obs_stats types) of the standardised transform, or None: `standardize` is None, a `mean_and_std` path or the
+    8 values; a checkpoint's "mean_and_std" is used when `standardize` is None and must equal it otherwise (ValueError)"""
+    from .obs_stats import check_mean_and_std, load_mean_and_std
+
+    if isinstance(standardize, (str, bytes)) or hasattr(standardize, "__fspath__"):
+        standardize = load_mean_and_std(standardize)
+    elif standardize is not None:
+        standardize = check_mean_and_std(standardize)
+    stored = None if not ckpt or ckpt.get("mean_and_std") is None else check_mean_and_std(ckpt["mean_and_std"])
+    if stored is not None and standardize is not None and [float(v) for v in stored] != [float(v) for v in standardize]:
+        raise ValueError(f"the checkpoint was trained on standardised observations with mean_and_std {[float(v) for v in stored]}, "
+                         f"not {[float(v) for v in standardize]}")
+    return stored if standardize is None else standardize
+
+
 def load_checkpoint(path_or_dict):
     import torch
 
@@ -94,12 +116,15 @@ def load_checkpoint(path_or_dict):
 class BatchedTrainer:
     def __init__(self, n_envs, scene="A", device=0, seed=0, batch_size=12, mem_size=None, updates_per_step=None, lr=1e-3, eps_start=EPS_START,
                  eps_end=EPS_END, eps_decay=EPS_DECAY, load=None, env_index_offset=None, n_total=None, process_group=None, chunk=64, max_draws=256,
-                 noise_std=0.001, log=None, prioritized=None, gamma=0.0, target_update=None, optimizer=None, momentum=0.9, accumulate=1):
+                 noise_std=0.001, log=None, prioritized=None, gamma=0.0, target_update=None, optimizer=None, momentum=0.9, accumulate=1,
+                 standardize=None):
         import torch
         import torch.distributed as dist
 
         self.gamma, self.target_update = check_bootstrap(gamma, target_update)
         _, self.accumulate, momentum = check_optimizer("adam" if optimizer is None else optimizer, accumulate, momentum)
+        ckpt = None if load is None else load_checkpoint(load)
+        self.standardize = resolve_standardize(standardize, ckpt)
         self.torch = torch
         self.pg = process_group
         rank, world = (dist.get_rank(process_group), dist.get_world_size(process_group)) if process_group is not None else (0, 1)
@@ -115,7 +140,6 @@ class BatchedTrainer:
         self.eps_start, self.eps_end, self.eps_decay = eps_start, eps_end, eps_decay
         self.chunk, self.max_draws, self.noise_std = int(chunk), int(max_draws), float(noise_std)
         self.log = log
-        ckpt = None if load is None else load_checkpoint(load)
         opt = {} if optimizer is None else {"optimizer": optimizer}
         if ckpt is None:
             self.learner = QNetLearner(None, device, lr=lr, seed=self.seed, process_group=process_group, momentum=momentum, accumulate=self.accumulate,
@@ -134,6 +158,8 @@ class BatchedTrainer:
         W, H = self.env.IMAGE_WIDTH, self.env.IMAGE_HEIGHT
         self.per = None
         nxt = {"next_obs": True} if self.gamma > 0 else {}  # at gamma = 0 the replays are built exactly as without bootstrapping
+        if self.standardize is not None:
+            nxt["standardize"] = self.standardize
         if prioritized is None:
             self.replay = ObservationReplay(mem, (H, W), device=self.dev, rng=random.Random(self.seed + rank), **nxt)
         else:
@@ -155,6 +181,8 @@ class BatchedTrainer:
     def acting_states(self, obs, step):
         """the keyed training transform of the observation: what the agent acts on and what the replay regenerates"""
         t = self.torch
+        if self.standardize is not None:
+            return self.learner.fw.obs_to_state_standard(obs, self.standardize, self.depth_threshold, self.noise_std, self.seed, step, self.genv)
         return self.learner.fw.obs_to_state_keyed(obs["rgb"], obs["depth"], self.genv, t.full((self.n_envs,), step, dtype=t.int64, device=self.dev),
                                                   self.seed, depth_threshold=self.depth_threshold, noise_std=self.noise_std)
 
@@ -296,9 +324,13 @@ class BatchedTrainer:
         return out
 
     def checkpoint(self):
-        """the dict the reference's main() saves (:560-572); with SGD also the learner's "learner_step" (QNetLearner.checkpoint)"""
+        """the dict the reference's main() saves (:560-572); with SGD also the learner's "learner_step" (QNetLearner.checkpoint), with
+        standardised observations also "mean_and_std" (8 Python floats: the checkpoint holds no numpy objects)"""
         ck = self.learner.checkpoint()
         extra = {"learner_step": ck["learner_step"]} if "learner_step" in ck else {}
+        stats = getattr(self, "standardize", None)  # absent on objects that only carry the checkpoint's fields
+        if stats is not None:
+            extra["mean_and_std"] = [float(v) for v in stats]
         return {"step": self.steps_done, "model_state_dict": ck["model_state_dict"], "optimizer_state_dict": ck["optimizer_state_dict"],
                 "epsilon": self.eps_threshold, **self.counters(), **extra}
 
@@ -338,10 +370,16 @@ def main(argv=None):
     p.add_argument("--momentum", type=float, default=0.9, help="SGD momentum of a fresh run (a loaded checkpoint keeps its own)")
     p.add_argument("--accumulate", type=int, default=1,
                    help="micro-batches of --batch-size per optimizer step, gradients summed (the reference's NUMBER_ACCUMULATIONS_BEFORE_UPDATE)")
+    p.add_argument("--standardize", default=None, metavar="PATH",
+                   help="a mean_and_std file (python -m mujoco_rl_ur5_b200.normalize): act and learn on standardised observations")
     a = p.parse_args(argv)
     try:
         check_bootstrap(a.gamma, a.target_update)
         check_optimizer(a.optimizer or "adam", a.accumulate, a.momentum)
+        if a.standardize is not None:
+            resolve_standardize(a.standardize)
+    except OSError as e:
+        p.error(f"--standardize: {e}")
     except ValueError as e:
         p.error(str(e))
     import os
@@ -362,7 +400,7 @@ def main(argv=None):
     tr = BatchedTrainer(a.envs, a.scene, device, seed=a.seed, batch_size=a.batch_size, mem_size=a.mem_size, updates_per_step=a.updates_per_step, lr=a.lr,
                         eps_start=a.eps_start, eps_end=a.eps_end, eps_decay=a.eps_decay, load=a.load, process_group=pg,
                         log=sys.stdout if (pg is None or dist.get_rank() == 0) else None, prioritized=per, gamma=a.gamma,
-                        target_update=a.target_update, optimizer=a.optimizer, momentum=a.momentum, accumulate=a.accumulate)
+                        target_update=a.target_update, optimizer=a.optimizer, momentum=a.momentum, accumulate=a.accumulate, standardize=a.standardize)
     try:
         tr.train(a.episodes, a.steps_per_episode)
         if a.out:

@@ -717,6 +717,124 @@ __global__ void k_obs_train_state(const unsigned char* __restrict__ rgb, const f
   }
 }
 
+// ---- transform_observation(normalize=False) (Grasping_Agent_multidiscrete.py:311-354): the observation standardised with the channel
+// statistics of normalize.py.  rgb stays in 0..255 (ToTensor does not scale float input), then (x - mean) / std; depth is clipped,
+// standardised, and the noise is added AFTER it (so noise_std is in standardised units).  Rows are addressed like k_obs_train_state.
+// The __f*_rn intrinsics are never contracted into an FMA, so every operation rounds as torch's sub_ / div_ / add do.
+struct StdParams { float mean[4], stdv[4]; };
+__global__ void k_obs_standard(const unsigned char* __restrict__ rgb, const float* __restrict__ depth, const long long* __restrict__ slot,
+                               const long long* __restrict__ env_index, const unsigned int* __restrict__ steps, unsigned int step, StdParams sp, float thr,
+                               float noise_std, unsigned long long seed, int B, int HW, float* __restrict__ state, bf16* __restrict__ state_nhwc) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (size_t)B * HW) return;
+  const int b = (int)(i / HW), p = (int)(i % HW);
+  const size_t src = (slot ? (size_t)slot[b] : (size_t)b) * HW + p;
+  const float r = __fdiv_rn(__fsub_rn((float)rgb[3 * src], sp.mean[0]), sp.stdv[0]);
+  const float g = __fdiv_rn(__fsub_rn((float)rgb[3 * src + 1], sp.mean[1]), sp.stdv[1]);
+  const float bl = __fdiv_rn(__fsub_rn((float)rgb[3 * src + 2], sp.mean[2]), sp.stdv[2]);
+  float d = __fdiv_rn(__fsub_rn(fminf(depth[src], thr), sp.mean[3]), sp.stdv[3]);
+  if (noise_std != 0.f) {  // noise_std * z is +0 for any finite z at noise_std = 0, so skipping the draw changes no bit
+    const unsigned long long env = env_index ? (unsigned long long)env_index[b] : (unsigned long long)b;
+    d = __fadd_rn(d, __fmul_rn(noise_std, obs_noise(seed, env, steps ? steps[b] : step, (uint32_t)p)));
+  } else {
+    d = __fadd_rn(d, 0.f);
+  }
+  if (state) {
+    float* out = state + (size_t)b * 4 * HW + p;
+    out[0] = r; out[HW] = g; out[2 * (size_t)HW] = bl; out[3 * (size_t)HW] = d;
+  }
+  if (state_nhwc) {
+    __nv_bfloat162* o = (__nv_bfloat162*)(state_nhwc + i * 4);
+    o[0] = __floats2bfloat162_rn(r, g); o[1] = __floats2bfloat162_rn(bl, d);
+  }
+}
+
+// ---- normalize.py (:20-66): per-channel mean and population std over every pixel of B observations.  RGB: exact integer sums of x and
+// x^2 (u64), so the mean is numpy's bit for bit and the std comes from the exact numerator n sum(x^2) - sum(x)^2 (128 bits).  Depth:
+// fp64, two passes (sum, then the sum of squared deviations from the fp64 mean).  Fixed grid (a function of n only), fixed per-thread
+// order, fixed tree in the block and one block for the final sum: the result does not depend on the device or the run.
+#define STATS_THREADS 256
+#define STATS_MAX_BLOCKS 2048
+struct StatPart { unsigned long long s[3], q[3]; double d; };
+__device__ __forceinline__ unsigned long long warp_sum_u64(unsigned long long v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+__device__ __forceinline__ double warp_sum_f64(double v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+// block sum of one thread's partial into `out` (valid in thread 0): butterfly in the warp, then the warps' sums in warp order
+__device__ void block_sum_part(StatPart& v, bool rgb, StatPart* out) {
+  __shared__ StatPart sw[STATS_THREADS / 32];
+  const int lane = threadIdx.x & 31, wp = threadIdx.x >> 5;
+  if (rgb)
+    for (int c = 0; c < 3; c++) { v.s[c] = warp_sum_u64(v.s[c]); v.q[c] = warp_sum_u64(v.q[c]); }
+  v.d = warp_sum_f64(v.d);
+  if (lane == 0) sw[wp] = v;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    StatPart t = sw[0];
+    for (int k = 1; k < STATS_THREADS / 32; k++) {
+      if (rgb)
+        for (int c = 0; c < 3; c++) { t.s[c] += sw[k].s[c]; t.q[c] += sw[k].q[c]; }
+      t.d += sw[k].d;
+    }
+    *out = t;
+  }
+}
+// pass 0: rgb sums and the depth sum; pass 1: sum of (d - mean)^2 with mean = fin->d / n
+__global__ void __launch_bounds__(STATS_THREADS) k_stats_part(const unsigned char* __restrict__ rgb, const float* __restrict__ depth, size_t n, int pass,
+                                                              const StatPart* __restrict__ fin, StatPart* __restrict__ part) {
+  StatPart v = {};
+  const size_t stride = (size_t)gridDim.x * STATS_THREADS;
+  if (pass == 0) {
+    for (size_t i = (size_t)blockIdx.x * STATS_THREADS + threadIdx.x; i < n; i += stride) {
+      const unsigned int r = rgb[3 * i], g = rgb[3 * i + 1], b = rgb[3 * i + 2];
+      v.s[0] += r; v.s[1] += g; v.s[2] += b;
+      v.q[0] += r * r; v.q[1] += g * g; v.q[2] += b * b;
+      v.d += (double)depth[i];
+    }
+  } else {
+    const double m = fin->d / (double)n;
+    for (size_t i = (size_t)blockIdx.x * STATS_THREADS + threadIdx.x; i < n; i += stride) {
+      const double e = (double)depth[i] - m;
+      v.d += e * e;
+    }
+  }
+  block_sum_part(v, pass == 0, part + blockIdx.x);
+}
+// one block: the partials of `nparts` blocks in block order -> fin (pass 0) or the eight statistics (pass 1)
+__global__ void __launch_bounds__(STATS_THREADS) k_stats_final(const StatPart* __restrict__ part, int nparts, size_t n, int pass, StatPart* __restrict__ fin,
+                                                               double* __restrict__ out) {
+  StatPart v = {};
+  for (int k = threadIdx.x; k < nparts; k += STATS_THREADS) {
+    for (int c = 0; c < 3; c++) { v.s[c] += part[k].s[c]; v.q[c] += part[k].q[c]; }
+    v.d += part[k].d;
+  }
+  __shared__ StatPart t;
+  block_sum_part(v, pass == 0, &t);
+  __syncthreads();
+  if (threadIdx.x != 0) return;
+  if (pass == 0) { *fin = t; return; }
+  const double nd = (double)n;  // n < 2^53: exact
+  for (int c = 0; c < 3; c++) {
+    const unsigned long long s = fin->s[c], q = fin->q[c];
+    out[c] = (double)s / nd;  // s < 2^53: the exact sum divided once, as np.mean of the uint8 channel
+    // num = n q - s^2 >= 0 exactly in 128 bits, rounded to double once (a sticky bit keeps the rounding of the shifted-out bits)
+    const unsigned __int128 num = (unsigned __int128)n * q - (unsigned __int128)s * s;
+    int sh = 0;
+    while ((num >> sh) >> 64) sh++;
+    unsigned long long top = (unsigned long long)(num >> sh);
+    if (sh && (num & (((unsigned __int128)1 << sh) - 1))) top |= 1ull;
+    out[4 + c] = sqrt(ldexp((double)top, sh) / (nd * nd));
+  }
+  out[3] = (double)(float)(fin->d / nd);
+  out[7] = (double)(float)sqrt(t.d / nd);
+}
+
 // ---- Grasp_Agent.epsilon_greedy (Grasping_Agent_multidiscrete.py:232-282) for a batch, one warp per env.  Greedy iff the keyed
 // uniform u > eps[b]; otherwise the reference's rejection sampling: candidate k (keyed draw j = 2 + k) is accepted when its pixel's
 // world z >= z_min.  The 32 lanes test candidates 32 at a time and the lowest accepted k wins, which is the first accepted candidate
@@ -790,6 +908,49 @@ extern "C" int gq_obs_to_state_keyed(const unsigned char* rgb, const float* dept
                                         scratch_red);
   k_obs_train_state<<<(unsigned)(((size_t)B * HW + 255) / 256), 256, 0, st>>>(rgb, depth, scratch_red, depth_threshold, noise_std, seed, slot, env_index, step,
                                                                               0u, jitter_out, order_out, B, HW, state, (bf16*)state_nhwc_bf16);
+  QCK(cudaGetLastError());
+  return 0;
+}
+extern "C" int gq_obs_to_state_standard(const unsigned char* rgb, const float* depth, const long long* slot, const long long* env_index,
+                                        const unsigned int* steps, unsigned int step, const float* mean_std, float depth_threshold, float noise_std,
+                                        unsigned long long seed, float* state, void* state_nhwc_bf16, int B, int HW, void* stream) {
+  if (!rgb || !depth || !mean_std || (!state && !state_nhwc_bf16) || B < 1 || HW < 1) {
+    snprintf(q_err, sizeof q_err, "gq_obs_to_state_standard: bad argument");
+    return -1;
+  }
+  StdParams sp;
+  for (int c = 0; c < 4; c++) {
+    sp.mean[c] = mean_std[c];
+    sp.stdv[c] = mean_std[4 + c];
+    if (!(sp.stdv[c] > 0.f)) {  // torchvision's Normalize refuses a zero std; a negative or NaN one is no standardisation either
+      snprintf(q_err, sizeof q_err, "gq_obs_to_state_standard: std of channel %d is %g, it must be > 0", c, (double)sp.stdv[c]);
+      return -1;
+    }
+  }
+  k_obs_standard<<<(unsigned)(((size_t)B * HW + 255) / 256), 256, 0, (cudaStream_t)stream>>>(rgb, depth, slot, env_index, steps, step, sp, depth_threshold,
+                                                                                             noise_std, seed, B, HW, state, (bf16*)state_nhwc_bf16);
+  QCK(cudaGetLastError());
+  return 0;
+}
+extern "C" size_t gq_obs_channel_stats_scratch_bytes(long long n_pixels) {
+  const long long blocks = (n_pixels + STATS_THREADS - 1) / STATS_THREADS;
+  return (size_t)((blocks < STATS_MAX_BLOCKS ? blocks : STATS_MAX_BLOCKS) + 1) * sizeof(StatPart);
+}
+extern "C" int gq_obs_channel_stats(const unsigned char* rgb, const float* depth, int B, int HW, void* scratch, double* out, void* stream) {
+  const size_t n = (size_t)B * (size_t)HW;
+  if (!rgb || !depth || !scratch || !out || B < 1 || HW < 1 || n >= ((size_t)1 << 44)) {  // n < 2^44 keeps 255 n < 2^53 and 255^2 n < 2^64
+    snprintf(q_err, sizeof q_err, "gq_obs_channel_stats: bad argument");
+    return -1;
+  }
+  const size_t want = (n + STATS_THREADS - 1) / STATS_THREADS;
+  const int blocks = (int)(want < STATS_MAX_BLOCKS ? want : STATS_MAX_BLOCKS);
+  StatPart* part = (StatPart*)scratch;
+  StatPart* fin = part + blocks;
+  cudaStream_t st = (cudaStream_t)stream;
+  for (int pass = 0; pass < 2; pass++) {
+    k_stats_part<<<blocks, STATS_THREADS, 0, st>>>(rgb, depth, n, pass, fin, part);
+    k_stats_final<<<1, STATS_THREADS, 0, st>>>(part, blocks, n, pass, fin, out);
+  }
   QCK(cudaGetLastError());
   return 0;
 }

@@ -24,7 +24,8 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 QLIB_PATH = os.path.join(_HERE, "csrc", "libgrasp_qnet.so")
 _QLIB = None
 QSYMBOLS = ["gq_last_error", "gq_version", "gq_conv_partials_floats", "gq_conv_tc", "gq_conv_tc_block_out", "gq_conv_first", "gq_maxpool", "gq_bn_act", "gq_upsample2x", "gq_head_up2", "gq_argmax", "gq_obs_to_state", "gq_obs_to_state_train", "gq_conv_tc_fused",
-            "gq_obs_to_state_keyed", "gq_sample_actions", "gq_head_max_target"]
+            "gq_obs_to_state_keyed", "gq_sample_actions", "gq_head_max_target", "gq_obs_to_state_standard", "gq_obs_channel_stats",
+            "gq_obs_channel_stats_scratch_bytes"]
 
 
 def load_qnet_library():
@@ -51,6 +52,10 @@ def load_qnet_library():
         L.gq_obs_to_state.argtypes = [P, P, F, P, P, I, I, P]
         L.gq_obs_to_state_train.argtypes = [P, P, F, F, C.c_uint64, P, C.c_uint32, P, P, P, P, P, I, I, P]
         L.gq_obs_to_state_keyed.argtypes = [P, P, P, P, P, F, F, C.c_uint64, P, P, P, P, P, I, I, P]
+        L.gq_obs_to_state_standard.argtypes = [P, P, P, P, P, C.c_uint32, P, F, F, C.c_uint64, P, P, I, I, P]
+        L.gq_obs_channel_stats_scratch_bytes.argtypes = [C.c_longlong]
+        L.gq_obs_channel_stats_scratch_bytes.restype = C.c_size_t
+        L.gq_obs_channel_stats.argtypes = [P, P, I, I, P, P, P]
         D = C.c_double
         L.gq_sample_actions.argtypes = [P, P, P, C.c_uint64, P, C.c_uint32, D, P, P, D, I, I, I, I, I, P, P, P, P]
         _QLIB = L
@@ -358,6 +363,34 @@ class QNetForward:
                                               int(seed) & (2 ** 64 - 1), self._p(red), self._p(fac), self._p(order), self._p(state), None, B, H * W,
                                               self._stream()), "gq_obs_to_state_keyed")
         return (state, fac, order) if return_draws else state
+
+    def obs_to_state_standard(self, obs, stats, depth_threshold=1.1, noise_std=0.001, seed=0, step=0, env_index=None, nhwc_bf16=False, slot=None):
+        """transform_observation(normalize=False) batched (gq_obs_to_state_standard): each channel standardised with `stats`, the 8 values
+        of normalize.py (obs_stats; mean r, g, b, depth, std r, g, b, depth, rounded to f32 as torchvision's Normalize does), rgb in
+        0..255, depth clipped at depth_threshold, then + noise_std * N(0, 1) keyed on (seed, env, step, pixel) as the training transform's
+        noise.  No ColorJitter.  Row b is image slot[b] of obs (None: b), keyed on env_index[b] (None: b) and step (an int, or [B] per
+        row).  noise_std=0 gives the deterministic part.  -> [B,4,H,W] f32, or ([B,4,H,W] f32, [B,H,W,4] bf16 NHWC) with nhwc_bf16=True"""
+        from .obs_stats import as_float32
+
+        t = self.torch
+        ms = as_float32(stats)
+        rgb, depth = obs["rgb"].contiguous(), obs["depth"].contiguous()
+        H, W = depth.shape[1], depth.shape[2]
+        sl = None if slot is None else t.as_tensor(slot).to(self.dev, t.int64).reshape(-1).contiguous()
+        B = depth.shape[0] if sl is None else sl.numel()
+        ei = None if env_index is None else t.as_tensor(env_index).to(self.dev, t.int64).reshape(B).contiguous()
+        st = None
+        if isinstance(step, (int, np.integer)):
+            step = int(step) & 0xFFFFFFFF
+        else:  # per row: the uint32 bit patterns
+            st = t.as_tensor(step).to(self.dev, t.int64).reshape(B).bitwise_and(0xFFFFFFFF).to(t.int32).contiguous()
+            step = 0
+        state = t.empty((B, 4, H, W), dtype=t.float32, device=self.dev)
+        nhwc = t.empty((B, H, W, 4), dtype=t.bfloat16, device=self.dev) if nhwc_bf16 else None
+        self._ck(self.L.gq_obs_to_state_standard(self._p(rgb), self._p(depth), self._p(sl), self._p(ei), self._p(st), step,
+                                                 ms.ctypes.data_as(C.c_void_p), float(depth_threshold), float(noise_std), int(seed) & (2 ** 64 - 1),
+                                                 self._p(state), self._p(nhwc), B, H * W, self._stream()), "gq_obs_to_state_standard")
+        return (state, nhwc) if nhwc_bf16 else state
 
     def sample_actions(self, depth, greedy_idx, eps, env_index, step, seed, camera, z_min, n_rot=6, max_draws=256):
         """epsilon-greedy selection (gq_sample_actions): depth [B,H,W] f32 of the current observation, greedy_idx [B] int32 (flat arg-max),

@@ -102,10 +102,18 @@ class ObservationReplay(_Ring):
 
     next_obs=True (bootstrapped learning, the reference's `next_state`, Grasping_Agent_multidiscrete.py:140-144,551-554): each
     transition also keeps the observation after its step and that observation's step key (280 004 B more at 200x200: rgb, depth,
-    uint32 key; the env is the transition's), and `sample` also returns the regenerated next states.  Off, nothing of it is stored."""
+    uint32 key; the env is the transition's), and `sample` also returns the regenerated next states.  Off, nothing of it is stored.
 
-    def __init__(self, size, image_hw=(200, 200), device="cuda", rng=None, seed=20, next_obs=False):
+    standardize=<8 values> (transform_observation(normalize=False), obs_stats): states are regenerated with the standardised transform
+    gq_obs_to_state_standard under the same keys instead; None (default) is the min-max training transform."""
+
+    def __init__(self, size, image_hw=(200, 200), device="cuda", rng=None, seed=20, next_obs=False, standardize=None):
         super().__init__(size, device, rng, seed)
+        if standardize is not None:
+            from .obs_stats import check_mean_and_std
+
+            standardize = check_mean_and_std(standardize)
+        self.standardize = standardize
         t = self.torch
         H, W = image_hw
         self.rgb = t.zeros((self.size, H, W, 3), dtype=t.uint8, device=self.device)
@@ -147,8 +155,11 @@ class ObservationReplay(_Ring):
             self.next_steps.index_copy_(0, idx, as_dev(self._key32(next_steps), t.int32))
 
     def _states(self, idx, fwd, seed, depth_threshold, noise_std, nxt=False):
-        """the keyed training transform of the stored (nxt: next) observations of slots idx"""
+        """the keyed training transform (or the standardised one) of the stored (nxt: next) observations of slots idx"""
         rgb, depth, steps = (self.next_rgb, self.next_depth, self.next_steps) if nxt else (self.rgb, self.depth, self.steps)
+        if self.standardize is not None:
+            return fwd.obs_to_state_standard({"rgb": rgb, "depth": depth}, self.standardize, depth_threshold, noise_std, seed, steps.index_select(0, idx),
+                                             self.envs.index_select(0, idx), slot=idx)
         return fwd.obs_to_state_keyed(rgb, depth, self.envs.index_select(0, idx), steps.index_select(0, idx), seed, slot=idx, depth_threshold=depth_threshold,
                                       noise_std=noise_std)
 
@@ -170,8 +181,8 @@ class PrioritizedObservationReplay(ObservationReplay):
     stratified (one uniform per 1/B of the total) and keyed on (seed, learner update, rank), so it needs no host generator and no
     host-to-device copy.  Priorities are not part of a checkpoint, like the stored transitions themselves."""
 
-    def __init__(self, size, image_hw=(200, 200), device="cuda", alpha=0.6, eps=1e-6, next_obs=False):
-        super().__init__(size, image_hw, device, rng=None, seed=None, next_obs=next_obs)  # the uniform generator is not used (nor the global one re-seeded)
+    def __init__(self, size, image_hw=(200, 200), device="cuda", alpha=0.6, eps=1e-6, next_obs=False, standardize=None):
+        super().__init__(size, image_hw, device, rng=None, seed=None, next_obs=next_obs, standardize=standardize)  # the uniform generator is not used (nor the global one re-seeded)
         from .qnet import load_qnet_library
         from .qnet_learn import _bind_learn
 

@@ -8,9 +8,9 @@
  * One handle per device; a handle is not thread-safe; launches go to the stream given at creation time
  * (0 = the legacy default stream).  N = number of environments of the handle.
  *
- * The library holds two builds of the engine (per-env workspace in shared memory / in HBM rows); ge_create picks one from the
- * scene's size (ge_size(h, 9) tells which), every other entry point forwards through the handle.  Handles of different scenes may
- * coexist in one process.
+ * The library holds two builds of the engine (one environment per warp / one environment per CTA of 4 warps, for scenes whose
+ * per-env workspace the warp-per-env build cannot hold); ge_create picks one from the scene's size (ge_size(h, 9) tells which), every
+ * other entry point forwards through the handle.  Handles of different scenes may coexist in one process.
  */
 #ifndef GRASP_ENGINE_H
 #define GRASP_ENGINE_H
@@ -40,14 +40,16 @@ const char* ge_version(void);
 /* mujoco_py.load_model_from_path + MjSim (MujocoController.py:33-36) + MJ_Controller.create_lists (:136-254):
  * model_blob = compiled scene (mujoco_rl_ur5_b200/model/blob.py), copied to the device; n_envs independent copies of the
  * scene are created at qpos0 with the reference PID gains.  stream: cudaStream_t cast to void* (NULL = default).
- * GE_ERR_MODEL for a scene with more than 256 geoms (the renderer's per-tile geom list).  Engines of one scene with different
- * workspace sizes (e.g. GE_MAXCON) may live side by side. */
+ * GE_ERR_MODEL for a scene with more than 256 geoms (the renderer's per-tile geom list), and for a kinematic tree that is not a
+ * single free body and has more than 8 dofs (the mass solve gives such a tree one 8-lane group; ge_last_error names the tree).  This
+ * check reads the host blob only and fails before any CUDA call.  Engines of one scene with different workspace sizes (e.g.
+ * GE_MAXCON) may live side by side. */
 int ge_create(const void* model_blob /*[host]*/, size_t nbytes, int n_envs, int device, void* stream, ge_handle* out);
 int ge_destroy(ge_handle h);
 
 /* model sizes: what = 0 nq, 1 nv, 2 nbody, 3 ngeom, 4 nu, 5 n_envs, 6 max contacts per env, 7 shared-memory bytes per env,
- * 8 environments (warps) per CTA of the sub-step kernel, 9 workspace placement (0 shared memory, 1 HBM rows: scenes whose per-env
- * workspace exceeds 227 KB, e.g. the 40-object scene), 10 hcap = doubles of the Newton Hessian block region in the workspace, 11 hfull =
+ * 8 environments per CTA of the sub-step kernel, 9 build (0 warp-per-env, 1 CTA-per-env: scenes whose warp-per-env workspace would
+ * exceed 227 KB, e.g. the 40-object scene), 10 hcap = doubles of the Newton Hessian block region in the workspace, 11 hfull =
  * nv (nv + 1) / 2 = doubles of one env's Hessian overflow row in HBM (a Hessian build whose blocks add up to more than hcap goes
  * there), 12 environments of the sub-step kernel resident per SM as granted by the occupancy API, 13 Hessian builds that used the
  * overflow row since ge_create (synchronises the engine's stream; saturates at INT_MAX).  Both builds read GE_HCAP at ge_create (hcap,

@@ -366,11 +366,10 @@ __device__ __noinline__ void group_chol_solve(const double* Hb, int lo, int nt, 
 }
 
 // x := (M + hdamp * diag(damping))^-1 x  for the block-diagonal (per kinematic tree) mass matrix, through dense per-tree
-// Cholesky factors in the (currently free) Hessian storage.  Replaces the tree-sparse L^T D L factor/solve when every tree fits
-// a lane group; returns false (nothing done) otherwise so that the caller can fall back.
-__device__ __noinline__ bool mass_block_solve(double* ws, double* x, double hdamp, int lane) {
+// Cholesky factors in the (currently free) Hessian storage.  Every non-simple tree fits a lane group: ge_create refuses a model
+// with a wider one.
+__device__ __noinline__ void mass_block_solve(double* ws, double* x, double hdamp, int lane) {
   const DevModel& m = c_m; const Layout& L = c_L;
-  for (int t = 0; t < m.ntree; t++) if (m.tree_dofnum[t] > GE_GROUP && !m.tree_simple[t]) return false;
   double* H = ws + L.H;
   const double* qM = ws + L.qM;
   // "simple" trees (free-floating single bodies): the block is a model constant, multiply by the precomputed inverse
@@ -413,7 +412,6 @@ __device__ __noinline__ bool mass_block_solve(double* ws, double* x, double hdam
     slot++;
   }
   gsync();
-  return true;
 }
 
 // x := -H^-1 g.  Uncoupled trees: 8-lane groups (group_chol_solve).  Coupled trees: right-looking dense Cholesky of the island's block

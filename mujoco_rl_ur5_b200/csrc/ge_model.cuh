@@ -40,15 +40,15 @@ struct DevModel {
 // workspace offsets, in doubles (ints live behind the doubles, offsets in ints from the int base)
 struct Layout {
   int qpos, qvel, qaccws, ctl;  // ctl: target[8] last_input[8] kp[8] ctrl[8]
-  int cdof, qM, qLD;
+  int cdof, qM;
   int qfrc_smooth, qacc_smooth, qfrc_constraint, qacc, Ma, grad, search, Mv;
   int con, cstride;             // contact records
   int sr;                       // simple rows: coefA coefB D aref jar jv  (6 x GE_MAXSR)
   int scratch;                  // phase-aliased region, see below
   int total_doubles;
   // --- aliases inside scratch: kinematics / dynamics phase
-  int lpos, lquat, janchor, jaxis, xpos, xquat, xmat, xipos, cinert, gpos, gmat, gcen;  // FK phase
-  int cvel, cacc, cfrc, cdofdot;                                                   // RNE phase (over lpos.. janchor.. xpos..)
+  int lpos, lquat, janchor, jaxis, xpos, xmat, cinert, gpos, gmat, gcen;  // FK phase
+  int cvel, cacc, cfrc, cdofdot;                                          // RNE phase (over lpos.. janchor.. xpos..)
   // --- aliases inside scratch: solver phase
   int H, Vb, Wb;
   // --- ints
@@ -57,7 +57,6 @@ struct Layout {
   int total_bytes;
   int maxcon, maxcand;          // capacity of the contact / candidate lists
   int fk_bytes;                 // bytes of the workspace prefix the kinematics stage touches (kinematics-only kernels)
-  int ws_global;                // 1: big-scene build (a CTA per env)
   int hcap;                     // doubles of the Hessian block region at L.H (= nv (nv + 1) / 2 when everything always fits)
   int hfull;                    // nv (nv + 1) / 2: size of the overflow row
   int i_hflag;                  // int slot: 1 while the Hessian blocks of the current build live in the overflow row

@@ -191,43 +191,6 @@ __device__ __noinline__ void stage_crb(double* ws, int lane) {
   gsync();
 }
 
-// L^T D L factorisation / solve of the tree-sparse mass matrix; one lane per kinematic tree (trees are independent)
-__device__ __noinline__ void factor_trees(double* LD, int lane) {
-  const DevModel& m = c_m;
-  LANE_LOOP(t, m.ntree) {
-    int lo = m.tree_dofadr[t], hi = lo + m.tree_dofnum[t];
-    for (int k = hi - 1; k >= lo; k--) {
-      int ak = m.dof_Madr[k], ki = 1;
-      double inv = 1.0 / LD[ak];
-      for (int i = m.dof_parentid[k]; i >= 0; i = m.dof_parentid[i], ki++) {
-        double a = LD[ak + ki] * inv;
-        int ai = m.dof_Madr[i], kj = ki, ij = 0;
-        for (int j = i; j >= 0; j = m.dof_parentid[j], kj++, ij++) LD[ai + ij] -= a * LD[ak + kj];
-        LD[ak + ki] = a;
-      }
-    }
-  }
-  gsync();
-}
-__device__ __noinline__ void solve_trees(const double* LD, double* x, int lane) {
-  const DevModel& m = c_m;
-  LANE_LOOP(t, m.ntree) {
-    int lo = m.tree_dofadr[t], hi = lo + m.tree_dofnum[t];
-    for (int k = hi - 1; k >= lo; k--) {
-      int ak = m.dof_Madr[k], ki = 1;
-      double xk = x[k];
-      for (int i = m.dof_parentid[k]; i >= 0; i = m.dof_parentid[i], ki++) x[i] -= LD[ak + ki] * xk;
-    }
-    for (int k = lo; k < hi; k++) x[k] /= LD[m.dof_Madr[k]];
-    for (int k = lo; k < hi; k++) {
-      int ak = m.dof_Madr[k], ki = 1;
-      double xk = x[k];
-      for (int i = m.dof_parentid[k]; i >= 0; i = m.dof_parentid[i], ki++) xk -= LD[ak + ki] * x[i];
-      x[k] = xk;
-    }
-  }
-  gsync();
-}
 // r = M v, one lane per dof (ancestors from the dof's own row, descendants from theirs)
 __device__ __noinline__ void mul_M(const double* qM, double* r, const double* v, int lane) {
   const DevModel& m = c_m;

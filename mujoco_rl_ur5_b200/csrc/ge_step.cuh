@@ -14,12 +14,9 @@ namespace ge {
 
 struct StepInfo { int ncon, nsr, niter, ncand, nmpr; };  // ncand, nmpr: see CollisionCounts
 
-// Stage barriers: when GE_STAGE_SYNC is on, all warps of the CTA (one env each) enter collision, the constraint solver and the
+// Stage barriers (warp-per-env build): all warps of the CTA (one env each) enter collision, the constraint solver and the
 // integrator together, so that the SM's instruction cache serves the (large) stage code once per CTA instead of once per warp.
 // Warps that do not step in an iteration must call stage_barriers_idle() to keep the barrier counts equal.
-#ifndef GE_STAGE_SYNC
-#define GE_STAGE_SYNC 1
-#endif
 #define GE_NUM_STAGE_BARRIERS (3 + GE_NEWTON_BARRIERS)
 // The warps of a CTA reach these barriers from DIFFERENT code locations (a stepping warp inside forward() / solve_newton(), a warp
 // whose environment does not step this iteration in stage_barriers_idle()).  That is legal for the unaligned PTX barrier
@@ -29,8 +26,8 @@ struct StepInfo { int ncon, nsr, niter, ncand, nmpr; };  // ncand, nmpr: see Col
 __device__ __forceinline__ void cta_barrier_unaligned() {
   asm volatile("barrier.sync 1, %0;" ::"r"((int)(blockDim.x * blockDim.y)) : "memory");
 }
-__device__ __forceinline__ void stage_barrier(bool sync) { if (GE_STAGE_SYNC && sync) cta_barrier_unaligned(); }
-__device__ __forceinline__ void stage_barriers_idle(bool on) { if (GE_STAGE_SYNC && on) for (int k = 0; k < GE_NUM_STAGE_BARRIERS; k++) cta_barrier_unaligned(); }
+__device__ __forceinline__ void stage_barrier(bool sync) { if (sync) cta_barrier_unaligned(); }
+__device__ __forceinline__ void stage_barriers_idle(bool on) { if (on) for (int k = 0; k < GE_NUM_STAGE_BARRIERS; k++) cta_barrier_unaligned(); }
 
 // debugging aid (GE_NANCHECK=1): first stage whose output holds a non-finite value -> one of status bits 8..15 (only the first is kept)
 __device__ __noinline__ void nan_probe(const double* a, int n, int lane, int* status, int bit) {
@@ -56,7 +53,6 @@ __device__ __noinline__ StepInfo forward(double* ws, int* wi, int lane, int* sta
     si.ncon = cc.ncon; si.ncand = cc.ncand; si.nmpr = cc.nmpr;
   }
   GE_CLK(SC_COLLISION);
-  if (dbg) nan_probe(ws + L.con, si.ncon * L.cstride < 16 * si.ncon ? 0 : 16 * 0 + si.ncon * 0, lane, status, 10);
   stage_rne(ws, lane);  // qfrc_smooth := bias
   stage_crb(ws, lane);
   GE_CLK(SC_RNE_CRB);
@@ -75,22 +71,15 @@ __device__ __noinline__ StepInfo forward(double* ws, int* wi, int lane, int* sta
   gsync();
   LANE_LOOP(d, m.nv) qas[d] = qfs[d];
   gsync();
-  // qacc_smooth = M^-1 qfrc_smooth: dense per-tree Cholesky in 8-lane groups (Hessian storage is free here); models with a
-  // tree wider than a lane group fall back to the tree-sparse L^T D L factorisation
-  if (!mass_block_solve(ws, qas, 0.0, lane)) {
-    LANE_LOOP(i, m.nM) ws[L.qLD + i] = ws[L.qM + i];
-    gsync();
-    factor_trees(ws + L.qLD, lane);
-    solve_trees(ws + L.qLD, qas, lane);
-  }
+  // qacc_smooth = M^-1 qfrc_smooth: dense per-tree Cholesky in 8-lane groups (Hessian storage is free here)
+  mass_block_solve(ws, qas, 0.0, lane);
   if (dbg) nan_probe(qas, m.nv, lane, status, 12);
   GE_CLK(SC_MASS);
   stage_barrier(sync);
   GE_CLK(SC_BARRIER);
   si.nsr = stage_constraints(ws, wi, lane, si.ncon, status);
   GE_CLK(SC_CONSTRAINTS);
-  if (dbg) nan_probe(ws + L.sr, 6 * GE_MAXSR * 0 + 4 * 0, lane, status, 13);
-  si.niter = solve_newton(ws, wi, lane, si.ncon, si.nsr, GE_STAGE_SYNC && sync);
+  si.niter = solve_newton(ws, wi, lane, si.ncon, si.nsr, sync);
   if (dbg) nan_probe(ws + L.qacc, m.nv, lane, status, 14);
   if (si.niter >= m.iterations) *status |= 4;
   LANE_LOOP(d, m.nv) ws[L.qaccws + d] = ws[L.qacc + d];
@@ -106,20 +95,10 @@ __device__ __noinline__ StepInfo sim_step(double* ws, int* wi, int lane, int* st
   stage_barrier(sync);
   GE_CLK(SC_BARRIER);
   double h = m.timestep;
-  double *acc = ws + L.grad, *qH = ws + L.qLD, *qvel = ws + L.qvel, *qpos = ws + L.qpos;
+  double *acc = ws + L.grad, *qvel = ws + L.qvel, *qpos = ws + L.qpos;
   LANE_LOOP(d, m.nv) acc[d] = ws[L.qfrc_smooth + d] + ws[L.qfrc_constraint + d];
   gsync();
-  if (!mass_block_solve(ws, acc, m.any_damping ? h : 0.0, lane)) {
-    if (m.any_damping) {
-      LANE_LOOP(i, m.nM) qH[i] = ws[L.qM + i];
-      gsync();
-      LANE_LOOP(d, m.nv) qH[m.dof_Madr[d]] += h * m.dof_damping[d];
-      gsync();
-      factor_trees(qH, lane);
-    }
-    gsync();
-    solve_trees(qH, acc, lane);
-  }
+  mass_block_solve(ws, acc, m.any_damping ? h : 0.0, lane);
   LANE_LOOP(d, m.nv) qvel[d] += h * acc[d];
   gsync();
   bool bad = false;

@@ -1,30 +1,25 @@
-// Two builds of the same engine source live in libgrasp_engine.so, selected per scene by ge_dispatch.cpp:
-//   variant 0 "smem": the per-env workspace is a slice of the CTA's shared memory.  Every workspace pointer provably derives
-//                     from the shared window, so the compiler emits LDS/STS in all stage functions (13 % fewer instructions
-//                     than generic loads, measured r01);
-//   variant 1 "hbm":  one workspace row per env in HBM (L1/L2-cached) for scenes whose workspace exceeds 227 KB (the 40-object
-//                     scene: the packed Newton Hessian alone is 247 KB).
+// Two builds of the same engine source live in libgrasp_engine.so, selected per scene by ge_dispatch.cpp.  Both keep each
+// environment's workspace in shared memory (every workspace pointer provably derives from the shared window, so the compiler emits
+// LDS/STS in all stage functions: 13 % fewer instructions than generic loads, measured r01):
+//   variant 0 "warp": one warp per environment, up to ten environments per SM;
+//   variant 1 "cta":  a whole CTA of 4 warps per environment, for scenes that variant 0 cannot hold in 227 KB per environment (the
+//                     40-object scene: the packed Newton Hessian alone is 247 KB).  The stage code is the same source: lane loops
+//                     stride by GE_LANES, `gsync()` is __syncthreads(), reductions go through shared memory, and the pieces that are
+//                     inherently warp-shaped (MPR on one geom pair, the 8-lane tree groups, one dense island factorisation) are dealt
+//                     out to the 4 warps.
 // The variant's namespace and its C entry points get a suffix; the public names of include/grasp_engine.h are the dispatcher's.
 #pragma once
 #ifndef GE_VARIANT
 #define GE_VARIANT 0
 #endif
 #if GE_VARIANT == 0
-#define ge ge_smem
-#define GE_API(n) n##_smem
-#define GE_WS_IN_HBM 0
+#define ge ge_warp
+#define GE_API(n) n##_warp
 #define GE_LANES 32   // threads that cooperate on one environment: one warp
 #else
-#define ge ge_hbm
-#define GE_API(n) n##_hbm
-#define GE_WS_IN_HBM 0  // (r02: the big-scene build keeps its workspace in shared memory too; only oversized Hessian builds overflow to HBM)
-// r02: the big-scene variant gives every environment a whole CTA of 4 warps.  The stage code is the same source: lane loops stride
-// by GE_LANES, `gsync()` is __syncthreads(), reductions go through shared memory, and the pieces that are inherently warp-shaped
-// (MPR on one geom pair, the 8-lane tree groups, one dense island factorisation) are dealt out to the 4 warps.
-#ifndef GE_BIG_LANES
-#define GE_BIG_LANES 128  // (-DGE_BIG_LANES=64 / 256: experiments with 2 / 8 warps per environment, tools/build_exp_libs.sh)
-#endif
-#define GE_LANES GE_BIG_LANES
+#define ge ge_cta
+#define GE_API(n) n##_cta
+#define GE_LANES 128  // threads that cooperate on one environment: one CTA of 4 warps
 #endif
 #define GE_NW (GE_LANES / 32)
 #define GE_ERR_TOO_LARGE (-100)  // internal: variant 0 cannot hold the scene, the dispatcher then creates variant 1

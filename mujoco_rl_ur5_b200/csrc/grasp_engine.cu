@@ -108,20 +108,16 @@ __device__ int env_take(const EnvArrays& E, int e, int nsub) {
 // Register budget.  Warp-per-env build: the workspace lets ten warps share an SM (ge_create), and the SM hands out registers per
 // quarter (16 384 each, in 256-register steps per warp): ten warps need three per quarter, i.e. <= 168 registers per thread.  Without a
 // cap ptxas takes 242 (2 warps per quarter = 8 per SM); `__maxnreg__(168)` costs a 1456 B stack (1296 B at 242) and small spills.
-// `__launch_bounds__(256)` alone gives 128 registers per thread (-DGE_V0_CAP_REGS); -DGE_RUN_MAXNREG=N tries another cap.
 // CTA-per-env build: two CTAs per SM is what the workspace allows; the bound keeps the register file from undercutting it.
+// Stage barriers (ge_step.cuh) keep the warps of a warp-per-env CTA in step; the CTA-per-env build has one env per CTA and none.
 #if GE_NW > 1
 #define GE_RUN_BOUNDS __launch_bounds__(GE_LANES, 2)
-#elif defined(GE_V0_CAP_REGS)
-#define GE_RUN_BOUNDS __launch_bounds__(256)
 #else
-#ifndef GE_RUN_MAXNREG
-#define GE_RUN_MAXNREG 168
-#endif
-#define GE_RUN_BOUNDS __maxnreg__(GE_RUN_MAXNREG)
+#define GE_RUN_BOUNDS __maxnreg__(168)
 #endif
 __global__ void GE_RUN_BOUNDS k_run(EnvArrays E, int n_env, int nsub, int quota, unsigned long long ticket_base, double base_x, double base_y,
-                                             double base_z, int stage_sync) {
+                                    double base_z) {
+  constexpr bool stage_sync = GE_NW == 1;
   extern __shared__ double smem[];
   const Layout& L = c_L;
   const int lane = threadIdx.x;
@@ -171,7 +167,7 @@ __global__ void GE_RUN_BOUNDS k_run(EnvArrays E, int n_env, int nsub, int quota,
     if (env < 0) break;                      // one env per CTA: `env` is the same in every thread
 #endif
     GE_CLK(SC_BARRIER);
-    if (env < 0) { stage_barriers_idle((stage_sync & 1) != 0); GE_CLK(SC_BARRIER); continue; }
+    if (env < 0) { stage_barriers_idle(stage_sync); GE_CLK(SC_BARRIER); continue; }
     bool stepped = false;
     // one iteration of the reference loop that ends in a physics step (or the env going idle)
     while (true) {
@@ -184,13 +180,13 @@ __global__ void GE_RUN_BOUNDS k_run(EnvArrays E, int n_env, int nsub, int quota,
       GE_CLK(SC_PID);
       if (delta < r.c.tol) { r.c.result = 1; r.c.reached = 1; }
       if (r.c.steps > r.c.maxsteps) { r.c.result = 2; r.c.active = 0; continue; }
-      if (!(stage_sync & 0x100)) sim_step(ws, wi, lane, &r.status, (stage_sync & 1) != 0);  // bit 8: GE_DBG_NOSTEP (scheduler-only experiments)
+      sim_step(ws, wi, lane, &r.status, stage_sync);
       stepped = true;
       r.c.steps++; r.nstep++;
       if (r.c.reached) r.c.active = 0;
       break;
     }
-    if (!stepped) { GE_CLK(SC_SCHED); stage_barriers_idle((stage_sync & 1) != 0); GE_CLK(SC_BARRIER); }
+    if (!stepped) { GE_CLK(SC_SCHED); stage_barriers_idle(stage_sync); GE_CLK(SC_BARRIER); }
     if (--left <= 0 || !running) {
       // a movement that just ended inside the last iteration still has to hand over to the program (no sub-step involved)
       while (!r.c.active && r.p.phase != PH_NONE) { if (!prog_advance(r.p, r.c, ws, lane, base, r.info, &r.reward)) break; }
@@ -517,14 +513,12 @@ struct ge_engine {
   cudaStream_t stream;
   DevModel hm;       // host copy of the struct holding DEVICE pointers
   Layout lay;
-  size_t ws_smem;    // dynamic shared memory per env of the stepping kernels (0: workspace in HBM)
   EnvArrays E;
   void* dblob;       // whole blob on the device
   std::vector<char> hblob;
   double base_pos[3];
   int64_t launches, substep_launches;
   int wpb;           // warps (= envs) per CTA of the sub-step kernel
-  int stage_sync;    // CTA barriers between the stages of a sub-step (instruction-cache sharing)
   int quota;         // iterations per visit of k_run's dynamic env scheduling
   int max_ctas;      // resident CTAs of k_run on this device (persistent grid)
   int groups_per_sm; // resident envs (groups) of k_run per SM that the occupancy API grants
@@ -536,18 +530,19 @@ struct ge_engine {
   void* state_scratch;             // [n_envs, R] records of ge_clone, allocated at its first call
 };
 
-static const void* blob_find(const std::vector<char>& b, const char* name, int64_t* count) {
-  int64_t n = *(const int64_t*)(b.data() + 8);
-  const BlobEntry* e = (const BlobEntry*)(b.data() + 24);
+static const void* blob_find(const char* b, const char* name, int64_t* count) {
+  int64_t n = *(const int64_t*)(b + 8);
+  const BlobEntry* e = (const BlobEntry*)(b + 24);
   for (int64_t i = 0; i < n; i++)
     if (strncmp(e[i].name, name, 32) == 0) {
       int64_t c = 1;
       for (int k = 0; k < e[i].ndim; k++) c *= e[i].shape[k];
       if (count) *count = c;
-      return b.data() + e[i].offset;
+      return b + e[i].offset;
     }
   return nullptr;
 }
+static const void* blob_find(const std::vector<char>& b, const char* name, int64_t* count) { return blob_find(b.data(), name, count); }
 static int64_t blob_off(const std::vector<char>& b, const char* name) {
   const void* p = blob_find(b, name, nullptr);
   return p ? (const char*)p - b.data() : -1;
@@ -558,13 +553,10 @@ static ge_engine* g_bound = nullptr;  // engine whose model / layout currently s
 
 static int align_up(int x, int a) { return (x + a - 1) / a * a; }
 
-static void make_layout(const DevModel& m, Layout& L, const int* tree_dofnum_h, const int* tree_simple_h, int ntree_dofnum_n, int maxcon, int hcap) {
+static void make_layout(const DevModel& m, Layout& L, int maxcon, int hcap) {
   int nb = m.nbody, nj = m.njnt, nv = m.nv, ng = m.ngeom;
   int o = 0;
   auto take = [&](int n) { int r = o; o += align_up(n, 2); return r; };
-  // the tree-sparse L^T D L factor is only needed when a tree is too wide for the lane-group mass solve
-  bool need_ld = false;
-  for (int t = 0; t < ntree_dofnum_n; t++) if (tree_dofnum_h[t] > 8 && !tree_simple_h[t]) need_ld = true;
   L.qpos = take(m.nq); L.qvel = take(nv); L.qaccws = take(nv); L.ctl = take(32);
   L.cdof = take(6 * nv);
   L.cstride = align_up(C_MU + 4 * m.maxdim - 1, 2);
@@ -582,7 +574,6 @@ static void make_layout(const DevModel& m, Layout& L, const int* tree_dofnum_h, 
   //                          body wrenches, dead while Hessian blocks are), over cinert and the RNE / CRB temporaries
   L.con = take(L.maxcon * L.cstride);
   L.qfrc_smooth = take(nv); L.qM = take(m.nM);
-  L.qLD = need_ld ? take(m.nM) : L.qM;
   L.scratch = o;
   int a = o;
   auto takeA = [&](int n) { int r = a; a += align_up(n, 2); return r; };
@@ -597,7 +588,6 @@ static void make_layout(const DevModel& m, Layout& L, const int* tree_dofnum_h, 
   a = nfk <= L.maxcon * L.cstride ? L.con : (endG > endT ? endG : endT);
   L.xpos = takeA(3 * nb); L.xmat = takeA(9 * nb); L.lpos = takeA(3 * nb); L.lquat = takeA(4 * nb); L.janchor = takeA(3 * nj); L.jaxis = takeA(3 * nj);
   const int endF = a;
-  L.xquat = L.xpos; L.xipos = L.xpos;  // (not stored any more)
   int b = L.scratch;
   auto takeB = [&](int n) { int r = b; b += align_up(n, 2); return r; };
   L.qacc_smooth = takeB(nv); L.qfrc_constraint = takeB(nv); L.qacc = takeB(nv);
@@ -614,7 +604,6 @@ static void make_layout(const DevModel& m, Layout& L, const int* tree_dofnum_h, 
 #else
   // CTA-per-env build: fixed arrays, then one scratch region aliased by phase
   L.qM = take(m.nM);
-  L.qLD = need_ld ? take(m.nM) : L.qM;
   L.qfrc_smooth = take(nv); L.qacc_smooth = take(nv); L.qfrc_constraint = take(nv); L.qacc = take(nv);
   L.Ma = take(nv); L.grad = take(nv); L.search = take(nv); L.Mv = take(nv);
   // list capacities: the 6-object scene settles at 17 contacts; its all-cube variant A1 (BASELINE configs 3-4) at 21-28 after
@@ -630,7 +619,6 @@ static void make_layout(const DevModel& m, Layout& L, const int* tree_dofnum_h, 
   auto takeA = [&](int n) { int r = a; a += align_up(n, 2); return r; };
   L.gpos = takeA(3 * ng); L.gmat = takeA(9 * ng); L.gcen = takeA(3 * ng);  // alive until the end of collision
   L.xpos = takeA(3 * nb); L.xmat = takeA(9 * nb);                            // alive until the end of stage_fk
-  L.xquat = L.xpos; L.xipos = L.xpos;                                        // (not stored any more)
   int a_local = a;
   L.lpos = takeA(3 * nb); L.lquat = takeA(4 * nb); L.janchor = takeA(3 * nj); L.jaxis = takeA(3 * nj);  // dead before cinert is written
   int endA1 = a;
@@ -662,13 +650,23 @@ static void make_layout(const DevModel& m, Layout& L, const int* tree_dofnum_h, 
   L.i_cand = takeI(L.maxcand); L.i_first = takeI(nv); L.i_tcoupled = takeI(m.ntree); L.i_tcount = takeI(m.ntree); L.i_tlist = takeI(m.ntree * GE_TLIST); L.i_island = takeI(m.ntree); L.i_hflag = takeI(1);
   L.total_ints = align_up(io, 4);
   L.total_bytes = L.total_doubles * 8 + L.total_ints * 4;
-  L.ws_global = 0;
   L.hovf_builds = nullptr;
 }
 
 extern "C" int ge_create(const void* model_blob, size_t nbytes, int n_envs, int device, void* stream, ge_handle* out) {
   if (!model_blob || nbytes < 32 || n_envs <= 0 || !out) return fail(GE_ERR_ARG, "ge_create: bad argument");
   if (memcmp(model_blob, "GEBLOB01", 8) != 0) return fail(GE_ERR_MODEL, "ge_create: not a model blob");
+  {  // the mass solve (mass_block_solve) gives each non-simple kinematic tree one group of GE_GROUP lanes
+    int64_t nd = 0, ns = 0;
+    const int32_t* dn = (const int32_t*)blob_find((const char*)model_blob, "tree_dofnum", &nd);
+    const int32_t* sm = (const int32_t*)blob_find((const char*)model_blob, "tree_simple", &ns);
+    for (int64_t t = 0; dn && sm && t < nd && t < ns; t++)
+      if (dn[t] > GE_GROUP && !sm[t]) {
+        snprintf(g_err, sizeof g_err, "ge_create: kinematic tree %d has %d dofs; a tree that is not a free body may have at most %d",
+                 (int)t, dn[t], GE_GROUP);
+        return GE_ERR_MODEL;
+      }
+  }
   CK(cudaSetDevice(device));
   ge_engine* h = new ge_engine();
   h->device = device; h->n_envs = n_envs; h->stream = (cudaStream_t)stream; h->launches = h->substep_launches = 0;
@@ -730,11 +728,15 @@ extern "C" int ge_create(const void* model_blob, size_t nbytes, int n_envs, int 
     memcpy(h->base_pos, bp, 24);
   }
   const int* tdn = (const int*)blob_find(B, "tree_dofnum", nullptr);
-  const int* tsi = (const int*)blob_find(B, "tree_simple", nullptr);
   // list capacities: the 6-object scene settles at 17 contacts; its all-cube variant A1 (BASELINE configs 3-4) at 21-28 after
   // stay(1000) over 200 oracle resets, and 121 oracle grasp attempts on A1 (cubes piling up in the drop bin) peak at 30
   // (tests/golden/scene_a1.json), so 32 holds both.  Piles of free objects need room for ~3 contacts per object
   const int maxcon_default = m.ntree <= 8 ? 32 : 128;
+  // test hooks: GE_MAXCON (16..512) sets the contact capacity, GE_HCAP the Hessian region (checked against each build's range below)
+  int maxcon_env = 0;
+  if (const char* ev = getenv("GE_MAXCON")) { int v = atoi(ev); if (v >= 16 && v <= 512) maxcon_env = v; }
+  const char* hcap_ev = getenv("GE_HCAP");
+  const long hcap_env = hcap_ev ? atol(hcap_ev) : 0;  // 0: unset (below every build's smallest region)
   int diag = 0;
   for (int t = 0; t < m.ntree; t++) diag += tdn[t] * (tdn[t] + 1) / 2;
   const int hfull = m.nv * (m.nv + 1) / 2;
@@ -745,7 +747,7 @@ extern "C" int ge_create(const void* model_blob, size_t nbytes, int n_envs, int 
     while (lo < hi) {
       int mid = (lo + hi + 1) / 2;
       Layout T;
-      make_layout(m, T, tdn, tsi, m.ntree, maxcon, mid);
+      make_layout(m, T, maxcon, mid);
       if ((long)T.total_bytes <= budget) lo = mid; else hi = mid - 1;
     }
     return lo;
@@ -756,24 +758,19 @@ extern "C" int ge_create(const void* model_blob, size_t nbytes, int n_envs, int 
   // overflow row in HBM.  The region must hold nt_update's contact and body wrenches, and the blocks of the mass solve (<= the tree
   // diagonal).
   {
-    int maxcon = maxcon_default;
-    if (const char* ev = getenv("GE_MAXCON")) { int v = atoi(ev); if (v >= 16 && v <= 512) maxcon = v; }
+    const int maxcon = maxcon_env ? maxcon_env : maxcon_default;
     int need_min = 6 * maxcon + 6 * m.nbody;
     if (diag > need_min) need_min = diag;
     int cap = fit(maxcon, (233472 - 2 * (1024 + (long)run_attr.sharedSizeBytes)) / 10);
     if (cap < need_min) cap = hfull;  // too large for ten per SM: the whole triangle, fewer envs per SM
-    make_layout(m, h->lay, tdn, tsi, m.ntree, maxcon, cap);
+    make_layout(m, h->lay, maxcon, cap);
     // GE_HCAP only moves the region of a scene this build holds anyway: a scene that needs the CTA-per-env build keeps it
-    if (const char* ev = getenv("GE_HCAP")) {
-      long v = atol(ev);
+    if (hcap_env >= need_min && hcap_env <= hfull && h->lay.total_bytes <= 227 * 1024) {
       Layout T;
-      if (v >= need_min && v <= hfull && h->lay.total_bytes <= 227 * 1024) {
-        make_layout(m, T, tdn, tsi, m.ntree, maxcon, (int)v);
-        if (T.total_bytes <= 227 * 1024) h->lay = T;
-      }
+      make_layout(m, T, maxcon, (int)hcap_env);
+      if (T.total_bytes <= 227 * 1024) h->lay = T;
     }
   }
-  h->lay.ws_global = 0;
   if (h->lay.total_bytes > 227 * 1024) { cudaFree(h->dblob); delete h; return fail(GE_ERR_TOO_LARGE, "per-env workspace exceeds shared memory"); }
 #else
   // CTA-per-env build: the workspace of ONE env per CTA in shared memory.  The Hessian block region is capped so that two CTAs share
@@ -781,8 +778,7 @@ extern "C" int ge_create(const void* model_blob, size_t nbytes, int n_envs, int 
   {
     // 112 contacts instead of the 128 of the r01 HBM layout: with 128 the phase-aliased workspace of the 40-object scene is 116.9 KB even
     // with an empty Hessian region - 3.3 KB over what lets two CTAs share an SM (settled piles hold 40-50 contacts; overflow is flagged)
-    int maxcon = maxcon_default > 112 ? 112 : maxcon_default;
-    if (const char* ev = getenv("GE_MAXCON")) { int v = atoi(ev); if (v >= 16 && v <= 512) maxcon = v; }
+    const int maxcon = maxcon_env ? maxcon_env : (maxcon_default > 112 ? 112 : maxcon_default);
     int need_min = diag + 6 * maxcon + 64;  // all trees uncoupled / the contact-wrench scratch of nt_update
     if (need_min > hfull) need_min = hfull;
     // the Hessian region shares the phase-aliased scratch with the kinematics arrays: largest cap whose layout fits the budget
@@ -790,10 +786,9 @@ extern "C" int ge_create(const void* model_blob, size_t nbytes, int n_envs, int 
     int cap = fit(maxcon, budget2);
     if (cap < need_min) cap = fit(maxcon, budget1);
     if (cap < need_min) { cudaFree(h->dblob); delete h; return fail(GE_ERR_MODEL, "model too large: per-env workspace exceeds shared memory even with one CTA per SM"); }
-    if (const char* ev = getenv("GE_HCAP")) { long v = atol(ev); if (v >= need_min && v <= hfull) cap = (int)v; }
-    make_layout(m, h->lay, tdn, tsi, m.ntree, maxcon, cap);
+    if (hcap_env >= need_min && hcap_env <= hfull) cap = (int)hcap_env;
+    make_layout(m, h->lay, maxcon, cap);
     if (h->lay.total_bytes > 227 * 1024) { cudaFree(h->dblob); delete h; return fail(GE_ERR_MODEL, "model too large: per-env workspace exceeds shared memory"); }
-    h->lay.ws_global = 1;
   }
 #endif
   if (h->lay.fk_bytes > 227 * 1024) { cudaFree(h->dblob); delete h; return fail(GE_ERR_MODEL, "model too large: kinematics workspace exceeds shared memory"); }
@@ -817,15 +812,7 @@ extern "C" int ge_create(const void* model_blob, size_t nbytes, int n_envs, int 
     }
     h->wpb = best;
   }
-  h->stage_sync = 1;  // lock-step warps of a CTA share instruction-cache lines (warp-per-env build)
-  if (const char* ev = getenv("GE_STAGE_SYNC")) h->stage_sync = atoi(ev) != 0;
-  if (GE_NW > 1) h->stage_sync = 0;
-  if (const char* ev = getenv("GE_DBG_NOSTEP")) if (atoi(ev) != 0) h->stage_sync |= 0x100;
   if (const char* ev = getenv("GE_WPB")) if (GE_NW == 1) { int v = atoi(ev); if (v >= 1 && v <= GE_MAX_WPB && v * h->lay.total_bytes <= 227 * 1024) h->wpb = v; }
-  h->ws_smem = (size_t)h->lay.total_bytes;
-  if (getenv("GE_VERBOSE"))
-    fprintf(stderr, "grasp_engine: %s build, workspace %d B per env (%d doubles + %d ints), contacts <= %d, Hessian region %d of %d doubles, %d env(s) per CTA\n",
-            GE_NW > 1 ? "CTA-per-env" : "warp-per-env", h->lay.total_bytes, h->lay.total_doubles, h->lay.total_ints, h->lay.maxcon, h->lay.hcap, h->lay.hfull, h->wpb);
   // The opt-in to more than 48 KB of dynamic shared memory belongs to the kernel, not to this engine: every engine of this build in the
   // process shares it.  Set to one engine's workspace, it would make the launches of another engine with a larger one fail.
   for (const void* k : {(const void*)k_debug, (const void*)k_step_open, (const void*)k_body_xpos, (const void*)k_render_fk}) {
@@ -842,15 +829,14 @@ extern "C" int ge_create(const void* model_blob, size_t nbytes, int n_envs, int 
   AL(E.prog_coords, double, N * 3); AL(E.prog_table, double, N); AL(E.reward, unsigned char, N); AL(E.status, int, N); AL(E.substeps, long long, N);
   AL(E.busy_count, int, 1); AL(E.lock, int, N); AL(E.owed, int, N); AL(E.done, int, N); AL(E.ticket, unsigned long long, 1);
   h->ticket_base = 0;
-  h->quota = 32;  // iterations per visit; H100, 4096 envs: see DESIGN.md section 4 (GE_QUOTA overrides)
-  if (const char* ev = getenv("GE_QUOTA")) { int v = atoi(ev); if (v >= 1) h->quota = v; }
+  h->quota = 32;  // iterations per visit; H100, 4096 envs: see DESIGN.md section 4
   {
     int per_sm = 0, sms = 0;
-    CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_run, GE_LANES * h->wpb, (size_t)h->wpb * h->ws_smem));
+    CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_run, GE_LANES * h->wpb, (size_t)h->wpb * h->lay.total_bytes));
     CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
     h->max_ctas = per_sm * sms > 0 ? per_sm * sms : 1;
     h->groups_per_sm = per_sm * h->wpb;
-    if (const char* ev = getenv("GE_MAXCTAS")) { int v = atoi(ev); if (v >= 1 && v < h->max_ctas) h->max_ctas = v; }  // experiments: fewer resident CTAs
+    if (const char* ev = getenv("GE_MAXCTAS")) { int v = atoi(ev); if (v >= 1 && v < h->max_ctas) h->max_ctas = v; }  // test hook: fewer resident CTAs
   }
   E.gws = nullptr;
   if (h->lay.hcap < h->lay.hfull) { AL(E.gws, double, N * (size_t)h->lay.hfull); }
@@ -895,7 +881,7 @@ extern "C" int ge_size(ge_handle h, int what) {
   if (!h) return GE_ERR_ARG;
   switch (what) {
     case 0: return h->hm.nq; case 1: return h->hm.nv; case 2: return h->hm.nbody; case 3: return h->hm.ngeom; case 4: return h->hm.nu;
-    case 5: return h->n_envs; case 6: return h->lay.maxcon; case 7: return h->lay.total_bytes; case 8: return h->wpb; case 9: return h->lay.ws_global;
+    case 5: return h->n_envs; case 6: return h->lay.maxcon; case 7: return h->lay.total_bytes; case 8: return h->wpb; case 9: return GE_NW > 1;
     case 10: return h->lay.hcap; case 11: return h->lay.hfull; case 12: return h->groups_per_sm;
     case 14: return 8 * rec_words(h->hm.nq, h->hm.nv);
     case 13: {  // Hessian builds that used the overflow row since ge_create (saturates at INT_MAX)
@@ -988,8 +974,8 @@ extern "C" int ge_run_async(ge_handle h, int substeps) {
   if (ctas > h->max_ctas) ctas = h->max_ctas;  // persistent grid: environments are handed to warps dynamically
   int quota = h->quota < substeps ? h->quota : substeps;
   CK(cudaMemsetAsync(h->E.done, 0, sizeof(int) * h->n_envs, h->stream));
-  k_run<<<ctas, blk, (size_t)h->wpb * h->ws_smem, h->stream>>>(h->E, h->n_envs, substeps, quota, h->ticket_base, h->base_pos[0], h->base_pos[1],
-                                                                h->base_pos[2], h->stage_sync);
+  k_run<<<ctas, blk, (size_t)h->wpb * h->lay.total_bytes, h->stream>>>(h->E, h->n_envs, substeps, quota, h->ticket_base, h->base_pos[0], h->base_pos[1],
+                                                                h->base_pos[2]);
   // every warp takes tasks until it has drawn one beyond the launch's range: n_env * visits real tasks + one overshoot per warp
   h->ticket_base += (unsigned long long)h->n_envs * ((substeps + quota - 1) / quota) + (unsigned long long)ctas * h->wpb;  // (one drawing group per env slot)
   h->launches++; h->substep_launches++;
@@ -1074,7 +1060,7 @@ extern "C" int ge_get_ctrl(ge_handle h, double* ctrl) {
 extern "C" int ge_step_open_loop(ge_handle h, int substeps, const uint8_t* env_mask) {
   if (!h || substeps <= 0) return fail(GE_ERR_ARG, "ge_step_open_loop: bad argument");
   if (bind(h)) return GE_ERR_CUDA;
-  k_step_open<<<h->n_envs, GE_LANES, h->ws_smem, h->stream>>>(h->E, h->n_envs, substeps, env_mask);
+  k_step_open<<<h->n_envs, GE_LANES, h->lay.total_bytes, h->stream>>>(h->E, h->n_envs, substeps, env_mask);
   h->launches++; h->substep_launches++;
   CK(cudaGetLastError());
   return GE_OK;
@@ -1123,7 +1109,7 @@ extern "C" int ge_debug_forward(ge_handle h, int env, const char* field, double*
   for (int i = 0; i < (int)(sizeof names / sizeof names[0]); i++) if (!strcmp(names[i], field)) f = i;
   if (f < 0) return fail(GE_ERR_ARG, "ge_debug_forward: unknown field %s", field);
   if (cap > (1 << 16)) cap = 1 << 16;
-  k_debug<<<1, GE_LANES, h->ws_smem, h->stream>>>(h->E, env, f, h->d_dbg, cap, h->d_nout);
+  k_debug<<<1, GE_LANES, h->lay.total_bytes, h->stream>>>(h->E, env, f, h->d_dbg, cap, h->d_nout);
   h->launches++;
   CK(cudaGetLastError());
   int n = 0;
@@ -1183,7 +1169,7 @@ extern "C" int ge_counters(ge_handle h, int64_t* kernel_launches, int64_t* subst
 
 #ifdef GE_STAGE_CLOCKS
 // profile builds only (ge_clocks.cuh): copies the per-warp-slot stage counters out, [GE_CLK_SLOTS][SC_NUM] u64, then zeroes them when
-// `reset` is set.  Exported under the variant's own name (ge_stage_clocks_smem / _hbm): the dispatcher does not know it.
+// `reset` is set.  Exported under the variant's own name (ge_stage_clocks_warp / _cta): the dispatcher does not know it.
 extern "C" int GE_API(ge_stage_clocks)(unsigned long long* out, int reset) {
   CK(cudaDeviceSynchronize());
   if (out) CK(cudaMemcpyFromSymbol(out, g_stage_clk, sizeof(g_stage_clk)));

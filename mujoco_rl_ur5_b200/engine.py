@@ -31,7 +31,7 @@ def load_library():
     """Load the CUDA engine; raises EngineError (never falls back) if it has not been built."""
     global _LIB
     if _LIB is None:
-        path = os.environ.get("GE_LIB", LIB_PATH)  # GE_LIB: alternative build of the same library (kernel experiments)
+        path = os.environ.get("GE_LIB", LIB_PATH)  # GE_LIB: alternative build of the same library (the -fmad=false test build, profile builds)
         if not os.path.exists(path):
             raise EngineError(f"{path} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'`")
         L = C.CDLL(path)

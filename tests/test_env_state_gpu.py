@@ -204,16 +204,16 @@ def test_refusals_leave_the_engine_unchanged(case, scene_a, scene_b):
     eng.close()
 
 
-def test_record_moves_between_the_two_builds(scene_a, monkeypatch):
+def test_record_moves_between_the_warp_and_cta_builds(scene_a, monkeypatch):
     blob = scene_a[0]
     q0, v0, coords, rot = _fixture("A")
     eng = _engine(blob, N)
     eng.set_state(q0, v0)
     _mid_attempt(eng, coords, rot)
     s = eng.snapshot()
-    monkeypatch.setenv("GE_WS_GLOBAL", "1")
+    monkeypatch.setenv("GE_CTA_PER_ENV", "1")
     hbm = _engine(blob, N)
-    monkeypatch.delenv("GE_WS_GLOBAL")
+    monkeypatch.delenv("GE_CTA_PER_ENV")
     assert eng.size(9) == 0 and hbm.size(9) == 1
     hbm.restore(s)
     assert hbm.snapshot().data.cpu().numpy().tobytes() == s.data.cpu().numpy().tobytes()

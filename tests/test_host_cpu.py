@@ -57,6 +57,23 @@ def test_cabi_library_exports_every_declared_symbol():
     assert b"blob" in lib.ge_last_error()
 
 
+def test_create_refuses_a_tree_wider_than_a_lane_group(scene_a):
+    """the mass solve gives every non-simple kinematic tree one 8-lane group: ge_create refuses a wider tree from the host blob,
+    before any CUDA call, so the refusal needs no device"""
+    from mujoco_rl_ur5_b200 import engine
+    from mujoco_rl_ur5_b200.model.blob import pack, unpack
+
+    arrays = unpack(scene_a[0])
+    assert arrays["tree_dofnum"][0] == 8 and not arrays["tree_simple"][0]  # the arm
+    arrays["tree_dofnum"][0] = 9
+    blob = pack(arrays)
+    lib = ctypes.CDLL(engine.LIB_PATH)
+    lib.ge_last_error.restype = ctypes.c_char_p
+    h = ctypes.c_void_p()
+    assert lib.ge_create(blob, len(blob), 4, 0, None, ctypes.byref(h)) == -3  # GE_ERR_MODEL
+    assert b"tree 0 has 9 dofs" in lib.ge_last_error()
+
+
 def test_engine_refuses_to_run_without_gpu():
     """no CPU fallback: constructing the engine without CUDA must fail loudly"""
     import torch

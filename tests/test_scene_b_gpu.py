@@ -140,9 +140,9 @@ def test_batched_env_scene_b_reset_and_step():
     env.close()
 
 
-def test_hbm_workspace_path_matches_shared_memory_path(scene_a):
-    """the same scene-A trajectory through both builds of the engine: warp-per-env with the workspace in shared memory, and
-    (GE_WS_GLOBAL=1) the big-scene build, a CTA of 4 warps per env.  Same arithmetic per item; the reductions over dofs / contacts
+def test_cta_per_env_build_matches_warp_per_env_build(scene_a):
+    """the same scene-A trajectory through both builds of the engine: warp-per-env, and (GE_CTA_PER_ENV=1) the big-scene build,
+    a CTA of 4 warps per env.  Same arithmetic per item; the reductions over dofs / contacts
     are summed in a different (each fixed) order, so the two agree to rounding, not bit for bit."""
     from mujoco_rl_ur5_b200.engine import BatchedEngine
 
@@ -151,11 +151,11 @@ def test_hbm_workspace_path_matches_shared_memory_path(scene_a):
     tgt = np.tile(HOME + np.array([0.3, 0.2, -0.2, 0.1, 0.1, 0.5, -0.1]), (4, 1))
     res = []
     for flag in ("0", "1"):
-        os.environ["GE_WS_GLOBAL"] = flag
+        os.environ["GE_CTA_PER_ENV"] = flag
         try:
             eng = BatchedEngine(blob, 4, 0)
         finally:
-            del os.environ["GE_WS_GLOBAL"]
+            del os.environ["GE_CTA_PER_ENV"]
         assert eng.size(9) == int(flag)
         eng.set_state(qpos)
         eng.move_group("All", tgt, 1e-7, 200)

@@ -34,7 +34,7 @@ def child(lib, steps, warmup):
     from mujoco_rl_ur5_b200.batched_env import BatchedGraspEnv
 
     L = engmod.load_library()
-    fn = L.ge_stage_clocks_smem
+    fn = L.ge_stage_clocks_warp
     fn.argtypes = [C.c_void_p, C.c_int]
     N, chunk = 4096, 256
     dev = torch.device("cuda", 0)

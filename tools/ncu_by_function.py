@@ -34,7 +34,7 @@ def function_ranges(so, kernel):
             continue
         if line.startswith("$"):
             name = line.strip().rstrip(":").split("$")[-1]
-            m = re.search(r"_ZN\d+ge(?:_smem|_hbm)?\d+([A-Za-z_0-9]+?)E", name)
+            m = re.search(r"_ZN\d+ge(?:_warp|_cta)?\d+([A-Za-z_0-9]+?)E", name)
             name = m.group(1) if m else name
             continue
         m = re.match(r"\s+/\*([0-9a-f]{4,})\*/", line)

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Small workload for compute-sanitizer (tools/sanitize.sh): every kernel of libgrasp_engine.so on a handful of environments —
-set_state, a movement with contacts (k_run: shared-memory variant for the 6-object scene, HBM-workspace variant for the 40-object
+set_state, a movement with contacts (k_run: warp-per-env build for the 6-object scene, CTA-per-env build for the 40-object
 scene), open-loop steps, IK, pixel_2_world, body_xpos, render.  Sizes are tiny because racecheck slows kernels down ~100x."""
 import sys, os
 import numpy as np

@@ -48,7 +48,7 @@ def ptxas_spills(log):
 
 
 def demangled_tail(name):
-    """_ZN7ge_smem5k_runE9EnvArrays... -> k_run;  __internal_accurate_pow -> itself"""
+    """_ZN7ge_warp5k_runE9EnvArrays... -> k_run;  __internal_accurate_pow -> itself"""
     m = re.match(r"_ZN\d+\w+?(\d+)(\w+)", name)
     if not m or not name.startswith("_ZN"):
         return name

@@ -10,9 +10,13 @@
 
 namespace ge {
 
+// The Newton Hessian build is split into its four parts: per-tree bookkeeping (coupling, contact membership, islands, block offsets),
+// the rows of M, the accumulation of the uncoupled trees' blocks and that of the island blocks.  SC_HESS_BUILDS / SC_HESS_COUPLED
+// count the builds, and those with at least one coupled tree (the island path).
 enum StageClock {
-  SC_PID, SC_FK, SC_COLLISION, SC_MPR, SC_RNE_CRB, SC_MASS, SC_CONSTRAINTS, SC_NEWTON, SC_HESSIAN, SC_CHOL, SC_LINESEARCH,
-  SC_NT_UPDATE, SC_EULER, SC_SCHED, SC_BARRIER, SC_SUBSTEPS, SC_WARM_FK, SC_WARM_RNE_CRB, SC_WARM_MULM, SC_MULM_COLD, SC_NUM
+  SC_PID, SC_FK, SC_COLLISION, SC_MPR, SC_RNE_CRB, SC_MASS, SC_CONSTRAINTS, SC_NEWTON, SC_HESS_LISTS, SC_HESS_MROWS, SC_HESS_TREES,
+  SC_HESS_ISLANDS, SC_CHOL, SC_LINESEARCH, SC_NT_UPDATE, SC_EULER, SC_SCHED, SC_BARRIER, SC_SUBSTEPS, SC_WARM_FK, SC_WARM_RNE_CRB,
+  SC_WARM_MULM, SC_MULM_COLD, SC_HESS_BUILDS, SC_HESS_COUPLED, SC_NUM
 };
 #define GE_CLK_SLOTS 4096
 

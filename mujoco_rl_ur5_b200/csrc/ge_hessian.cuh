@@ -2,14 +2,15 @@
 //
 // The mass matrix is block diagonal over kinematic trees (the arm + one block per object).  A contact couples two trees
 // only when both of its bodies are dynamic and belong to different trees.  Trees that no such contact (or equality row)
-// touches are "uncoupled": their Hessian block is assembled, factorised and solved by an 8-lane group each, several trees at a
-// time.  Coupled trees (e.g. arm + grasped object, touching objects of a pile) form connected components ("islands"); the Hessian
+// touches are "uncoupled": their Hessian block is assembled, factorised and solved in the registers of an 8-lane group each, several
+// trees at a time (tree_solve), and never stored.  Coupled trees (e.g. arm + grasped object, touching objects of a pile) form connected components ("islands"); the Hessian
 // is block diagonal over islands and each island is factorised as ONE dense matrix by one warp.
 //
 // Storage (r02): nothing is kept at global dof indices any more.  The region L.H (nv (nv + 1) / 2 doubles, the size of the full
 // packed triangle, which is an upper bound of what follows) is handed out per Hessian build: one packed lower-triangular BLOCK per
 // uncoupled tree (n_t (n_t + 1) / 2) and one per island (n_isl (n_isl + 1) / 2, island-local row order = ascending dof order),
-// back to back.  Entry (i, j) of a block lives at  off + r (r + 1) / 2 + c  with r, c the block-local indices, so the factorisation
+// back to back (an uncoupled tree's block is only counted: its offset, the total and the overflow decision stay those of the full layout,
+// but tree_solve keeps the block in registers).  Entry (i, j) of a block lives at  off + r (r + 1) / 2 + c  with r, c the block-local indices, so the factorisation
 // loops run over dense local indices (the r01 version indexed the global triangle through a dof list: 247 KB of scattered entries
 // per environment in the 40-object scene, ~12 integer instructions per multiply-add).  Included by ge_solver.cuh.
 #pragma once
@@ -65,33 +66,49 @@ __device__ __noinline__ void build_hessian(double* ws, int* wi, int ncon, int ns
   const int wl = lane & 31, wid = lane >> 5;
   int* tcoupled = wi + L.i_tcoupled;
   int *tcount = wi + L.i_tcount, *tlist = wi + L.i_tlist, *island = wi + L.i_island;  // tcount: #contacts (uncoupled) / first island row (coupled)
+  GE_CLK_COUNT(SC_HESS_BUILDS);
   // ---- which trees are coupled to another tree by an active constraint (trees wider than a lane group take the coupled path too)
   LANE_LOOP(t, m.ntree) { tcoupled[t] = m.tree_dofnum[t] > GE_GROUP ? 1 : 0; island[t] = t; }
   gsync();
-  LANE_LOOP(ci, ncon) {
-    if (!wi[L.i_cact + ci]) continue;
-    int t1 = wi[L.i_ct1 + ci], t2 = wi[L.i_ct2 + ci];
-    if (t1 >= 0 && t2 >= 0 && t1 != t2) { tcoupled[t1] = 1; tcoupled[t2] = 1; }
-  }
   LANE_LOOP(i, nsr) {
     if (!wi[L.i_sract + i]) continue;
     int A = wi[L.i_srA + i], B = wi[L.i_srB + i];
     if (B >= 0 && m.dof_treeindex[A] != m.dof_treeindex[B]) { tcoupled[m.dof_treeindex[A]] = 1; tcoupled[m.dof_treeindex[B]] = 1; }
   }
-  gsync();
-  // ---- per-tree lists of the active contacts that live entirely inside one uncoupled tree (one lane per tree scans the contacts)
-  LANE_LOOP(t, m.ntree) {
-    int cnt = 0;
-    if (!tcoupled[t]) {
-      NO_UNROLL for (int ci = 0; ci < ncon; ci++)
-        if (wi[L.i_cact + ci] && (wi[L.i_ct1 + ci] == t || wi[L.i_ct2 + ci] == t)) { if (cnt < GE_TCAP) tlist[t * GE_TLIST + cnt] = ci; cnt++; }
-      if (cnt > GE_TCAP) { tcoupled[t] = 1; cnt = 0; }  // too many contacts for the list: this tree takes the coupled path
+  // ---- per-tree lists of the active contacts, in one pass over the contacts.  Thread `lane` owns trees lane and lane + GE_LANES
+  // (ntree <= 2 * GE_LANES is checked at ge_create).  Every warp goes over all contacts, 32 at a time, and one ballot per tree it owns
+  // marks the chunk's active contacts of that tree: the contacts enter the tree's list (in contact order) at their rank in the ballot,
+  // and the owner counts them and notes whether one of them couples the tree to another tree.
+  const int ta = lane, tb = lane + GE_LANES;
+  int cnta = 0, cntb = 0;
+  bool cpa = false, cpb = false;
+  NO_UNROLL for (int cb = 0; cb < ncon; cb += 32) {
+    const int ci = cb + wl;
+    int t1 = -1, t2 = -1;
+    if (ci < ncon && wi[L.i_cact + ci]) { t1 = wi[L.i_ct1 + ci]; t2 = wi[L.i_ct2 + ci]; }
+    const unsigned cpl = __ballot_sync(FULL, t1 >= 0 && t2 >= 0 && t1 != t2), below = (1u << wl) - 1u;
+#pragma unroll
+    for (int s = 0; s < 2; s++) {  // the trees of my warp: lane wl owns tree tbase + wl
+      const int tbase = s * GE_LANES + (lane & ~31), tend = min(m.ntree, tbase + 32);
+      NO_UNROLL for (int t = tbase; t < tend; t++) {
+        const unsigned b = __ballot_sync(FULL, t1 == t || t2 == t);
+        const int base = __shfl_sync(FULL, s ? cntb : cnta, t - tbase);
+        if ((b >> wl) & 1u) { const int pos = base + __popc(b & below); if (pos < GE_TCAP) tlist[t * GE_TLIST + pos] = ci; }
+        if (t - tbase == wl) {
+          if (s) { cntb += __popc(b); cpb |= (b & cpl) != 0; }
+          else { cnta += __popc(b); cpa |= (b & cpl) != 0; }
+        }
+      }
     }
-    tcount[t] = cnt;
   }
   gsync();
-  bool any_coupled = false;
-  for (int t = 0; t < m.ntree; t++) any_coupled |= tcoupled[t] != 0;
+  // a tree with more contacts than GE_TCAP takes the coupled path
+  bool my_coupled = false;
+  if (ta < m.ntree) { const bool c = tcoupled[ta] || cpa || cnta > GE_TCAP; tcoupled[ta] = c; tcount[ta] = c ? 0 : cnta; my_coupled |= c; }
+  if (tb < m.ntree) { const bool c = tcoupled[tb] || cpb || cntb > GE_TCAP; tcoupled[tb] = c; tcount[tb] = c ? 0 : cntb; my_coupled |= c; }
+  const bool any_coupled = group_any(my_coupled);
+  gsync();
+  if (any_coupled) GE_CLK_COUNT(SC_HESS_COUPLED);
   // ---- islands of the coupled trees.  Label propagation: every tree starts with its own index, edges pull both ends to the smaller
   // label until nothing changes (the fixed point - the smallest tree index of the component - does not depend on the update order).
   if (any_coupled) {
@@ -122,7 +139,6 @@ __device__ __noinline__ void build_hessian(double* ws, int* wi, int ncon, int ns
     // depending on when the line is evicted (r02d: garbage Hessian blocks -> non-finite states under load; gone with -Xptxas -dlcm=cg).
     // Read the final labels past L1 once and write them back with ordinary stores, which L1 does track.
     {
-      const int ta = lane, tb = lane + GE_LANES;  // (ntree <= 2 * GE_LANES is checked at ge_create)
       const int la = ta < m.ntree ? ((volatile int*)island)[ta] : 0, lb = tb < m.ntree ? ((volatile int*)island)[tb] : 0;
       gsync();
       if (ta < m.ntree) island[ta] = la;
@@ -141,27 +157,27 @@ __device__ __noinline__ void build_hessian(double* ws, int* wi, int ncon, int ns
     gsync();
   }
   // ---- block offsets: trees in ascending order, an uncoupled tree takes its own block, an island takes its block at its representative
-  LANE_LOOP(t, m.ntree) {
-    int off = 0;
-    const int stop = tcoupled[t] ? island[t] : t;
-    for (int u = 0; u < stop; u++) {
+  // (exclusive prefix sum of the block sizes in tree order; a coupled tree then takes the offset of its island's representative)
+  {
+    auto block_size = [&](int u) -> int {
+      if (u >= m.ntree) return 0;
       int n;
       if (!tcoupled[u]) n = m.tree_dofnum[u];
       else if (island[u] == u) n = tlist[u * GE_TLIST];
-      else continue;
-      off += n * (n + 1) / 2;
+      else return 0;
+      return n * (n + 1) / 2;
+    };
+    int tot, offb = 0;
+    const int offa = group_exscan(block_size(ta), lane, tot);
+    if (m.ntree > GE_LANES) { int tot2; offb = tot + group_exscan(block_size(tb), lane, tot2); tot += tot2; }
+    if (ta < m.ntree) T_HOFF(tlist, ta) = offa;
+    if (tb < m.ntree) T_HOFF(tlist, tb) = offb;
+    if (any_coupled) {
+      gsync();
+      if (ta < m.ntree && tcoupled[ta] && island[ta] != ta) T_HOFF(tlist, ta) = T_HOFF(tlist, island[ta]);  // (representatives are not rewritten)
+      if (tb < m.ntree && tcoupled[tb] && island[tb] != tb) T_HOFF(tlist, tb) = T_HOFF(tlist, island[tb]);
     }
-    T_HOFF(tlist, t) = off;
-  }
-  {  // total size of this build's blocks (every thread adds up the same list)
-    int tot = 0;
-    for (int u = 0; u < m.ntree; u++) {
-      int n;
-      if (!tcoupled[u]) n = m.tree_dofnum[u];
-      else if (island[u] == u) n = tlist[u * GE_TLIST];
-      else continue;
-      tot += n * (n + 1) / 2;
-    }
+    // total size of this build's blocks
     const bool ovf = tot > L.hcap;
     if (ovf) H = g_hovf[threadIdx.y];
     if (lane == 0) {
@@ -186,68 +202,20 @@ __device__ __noinline__ void build_hessian(double* ws, int* wi, int ncon, int ns
   }
 #endif
   gsync();
-  // ---- rows of M: zero fill of the whole block row, then the tree-sparse row of qM
+  GE_CLK(SC_HESS_LISTS);
+  if (!any_coupled) return;
+  // ---- rows of M of the coupled trees: zero fill of the whole island row, then the tree-sparse row of qM
   LANE_LOOP(i, m.nv) {
     const int t = m.dof_treeindex[i], lo = m.tree_dofadr[t];
-    const int r0 = tcoupled[t] ? tcount[t] : 0, r = r0 + i - lo;
+    if (!tcoupled[t]) continue;
+    const int r0 = tcount[t], r = r0 + i - lo;
     double* row = H + T_HOFF(tlist, t) + r * (r + 1) / 2;
     NO_UNROLL for (int j = 0; j <= r; j++) row[j] = 0;
     int a = m.dof_Madr[i], k = 0;
     NO_UNROLL for (int j = i; j >= 0; j = m.dof_parentid[j], k++) row[r0 + j - lo] = qM[a + k];
   }
   gsync();
-  // ---- uncoupled trees: one 8-lane group per tree, GE_LANES / 8 trees at a time, every group walking ITS OWN contact list so that
-  // the groups really run concurrently (same instruction stream, different contacts).  Lane l of a group owns dof lo + l; the
-  // contact's Jacobian block is rebuilt in registers and J^T W J is added to the tree's dense block through shuffles.
-  {
-    const int g = lane / GE_GROUP, l = lane % GE_GROUP, gw = wl & ~(GE_GROUP - 1);  // gw: first lane of my group inside my warp
-    for (int t0 = 0; t0 < m.ntree; t0 += GE_LANES / GE_GROUP) {
-      const int t = t0 + g;
-      const bool valid = t < m.ntree && !tcoupled[t];
-      const int lo = valid ? m.tree_dofadr[t] : 0, nt = valid ? m.tree_dofnum[t] : 0, cnt = valid ? tcount[t] : 0;
-      double* Hb = H + (valid ? T_HOFF(tlist, t) : 0);
-      const int mydof = lo + l;
-      int maxcnt = cnt;
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) maxcnt = max(maxcnt, __shfl_xor_sync(FULL, maxcnt, o));
-      NO_UNROLL for (int n = 0; n < maxcnt; n++) {
-        const bool act = n < cnt && l < nt;
-        double J[6] = {0, 0, 0, 0, 0, 0}, tw[6] = {0, 0, 0, 0, 0, 0};
-        if (act) {
-          const int ci = tlist[t * GE_TLIST + n];
-          const double* c = ws + L.con + ci * L.cstride;
-          const int dim = wi[L.i_cdim + ci], t1 = wi[L.i_ct1 + ci], t2 = wi[L.i_ct2 + ci];
-          // sign of my dof in the contact's dof list (chains of both bodies minus their common ancestors) from the per-body
-          // bit masks over the tree-local dof index
-          unsigned m1 = t1 == t ? (unsigned)m.body_chainmask[wi[L.i_cb1 + ci]] : 0u, m2 = t2 == t ? (unsigned)m.body_chainmask[wi[L.i_cb2 + ci]] : 0u;
-          double sgn = ((m2 & ~m1) >> l & 1u) ? 1.0 : (((m1 & ~m2) >> l & 1u) ? -1.0 : 0.0);
-          if (sgn != 0) { jac_column(c, dim, cdof + 6 * mydof, sgn, J); weight_column(c, dim, wi[L.i_cact + ci], J, tw); }
-        }
-        for (int f = 0; f < GE_GROUP; f++) {
-          double h = 0;
-          NO_UNROLL for (int k = 0; k < m.maxdim; k++) h += tw[k] * __shfl_sync(FULL, J[k], gw + f);
-          if (act && l >= f && f < nt && h != 0.0) Hb[HIDX(l, f)] += h;
-        }
-      }
-      __syncwarp();
-      if (valid && l == 0)
-        for (int i = 0; i < nsr; i++) {
-          if (!wi[L.i_sract + i]) continue;
-          int A = wi[L.i_srA + i], B = wi[L.i_srB + i];
-          if (m.dof_treeindex[A] != t) continue;
-          double D = srv(ws, SR_D, i), ca = srv(ws, SR_CA, i), cb = srv(ws, SR_CB, i);
-          Hb[HIDX(A - lo, A - lo)] += D * ca * ca;
-          if (B >= 0) {
-            Hb[HIDX(B - lo, B - lo)] += D * cb * cb;
-            int hi = A > B ? A : B, lw = A > B ? B : A;
-            Hb[HIDX(hi - lo, lw - lo)] += D * ca * cb;
-          }
-        }
-      __syncwarp();
-    }
-  }
-  gsync();
-  if (!any_coupled) return;
+  GE_CLK(SC_HESS_MROWS);
   // ---- coupled trees: warp-cooperative accumulation, one lane per dof of the contact; a contact belongs to the warp that owns its
   // island.  Block-local row of dof d of tree t: tcount[t] + d - tree_dofadr[t].
   NO_UNROLL for (int ci = 0; ci < ncon; ci++) {
@@ -316,17 +284,16 @@ __device__ __noinline__ void build_hessian(double* ws, int* wi, int ncon, int ns
   gsync();
 }
 
-// Dense Cholesky + forward/backward substitution of one tree block (packed lower triangle `Hb` of nt <= GE_GROUP rows, dofs lo ..
-// lo + nt - 1) inside an 8-lane group, entirely in REGISTERS: lane l loads row l of the block once (static register indices, the loops
-// are fully unrolled), the factorisation exchanges pivots / column entries through shuffles, nothing is written back to the matrix
-// (the factor is used exactly once).  Rows l >= nt are padded with the identity.  x[lo + l] := sign * (H_block^-1 g)[l].
+// Dense Cholesky + forward/backward substitution of one tree block (nt <= GE_GROUP rows, dofs lo .. lo + nt - 1) inside an 8-lane
+// group, entirely in REGISTERS: lane l holds row l of the block's lower triangle in r[] (static register indices, the loops are fully
+// unrolled; rows l >= nt padded with the identity), the factorisation exchanges pivots / column entries through shuffles, nothing is
+// written back to the matrix (the factor is used exactly once).  x[lo + l] := sign * (H_block^-1 g)[l].
 // (A shared-memory version spends most of its instructions in packed-index arithmetic, LDS/STS and three __syncwarp per column.)
-__device__ __noinline__ void group_chol_solve(const double* Hb, int lo, int nt, int l, unsigned gmask, const double* g_, double* x, double sign) {
+__device__ __forceinline__ void group_chol_regs(double (&r)[GE_GROUP], int lo, int nt, int l, unsigned gmask, const double* g_, double* x,
+                                                double sign) {
   const int row = lo + l;
   const bool mine = l < nt;
-  double r[GE_GROUP], inv[GE_GROUP];
-#pragma unroll
-  for (int j = 0; j < GE_GROUP; j++) r[j] = (mine && j <= l) ? Hb[HIDX(l, j)] : (j == l ? 1.0 : 0.0);
+  double inv[GE_GROUP];
   // right-looking Cholesky: after step j, r[j] holds L[l][j] (rows l > j), later columns carry the Schur complement.  Only 1 / L[j][j]
   // is ever needed (scaling of column j, the two substitutions), so the pivot is one reciprocal square root (rsqrt: <= 1 ulp).
 #pragma unroll
@@ -363,6 +330,85 @@ __device__ __noinline__ void group_chol_solve(const double* Hb, int lo, int nt, 
     else if (l < i) y -= lil * xi;
   }
   if (mine) x[row] = sign * y;
+}
+// the same for a block stored as a packed lower triangle `Hb`: lane l loads row l once
+__device__ __noinline__ void group_chol_solve(const double* Hb, int lo, int nt, int l, unsigned gmask, const double* g_, double* x, double sign) {
+  const bool mine = l < nt;
+  double r[GE_GROUP];
+#pragma unroll
+  for (int j = 0; j < GE_GROUP; j++) r[j] = (mine && j <= l) ? Hb[HIDX(l, j)] : (j == l ? 1.0 : 0.0);
+  group_chol_regs(r, lo, nt, l, gmask, g_, x, sign);
+}
+
+// x := -H^-1 g on the uncoupled trees.  One 8-lane group per tree, GE_LANES / 8 trees at a time; lane l of a group owns dof lo + l and
+// keeps row l of the tree's Hessian block in registers: the row of M (through the dense qM index table dof_Mcol), then every active
+// contact of the tree in ascending contact index - the contact's Jacobian block is rebuilt in registers and J^T W J is added through
+// shuffles, every group walking ITS OWN contacts so that the groups really run concurrently - then the active simple rows in row order,
+// and the block is factorised and solved where it is (group_chol_regs).  Each entry receives the same additions, in the same order, as
+// the stored block of the island path would.  The contact lists are build_hessian's.
+__device__ __noinline__ void tree_solve(double* ws, const int* wi, int ncon, int nsr, double* x, const double* g_, int lane) {
+  const DevModel& m = c_m; const Layout& L = c_L;
+  const double *qM = ws + L.qM, *cdof = ws + L.cdof;
+  const int *tcoupled = wi + L.i_tcoupled, *tcount = wi + L.i_tcount, *tlist = wi + L.i_tlist;
+  const int wl = lane & 31, g = lane / GE_GROUP, l = lane % GE_GROUP, gw = wl & ~(GE_GROUP - 1);  // gw: first lane of my group inside my warp
+  const unsigned gmask = ((1u << GE_GROUP) - 1u) << gw;
+  for (int t0 = 0; t0 < m.ntree; t0 += GE_LANES / GE_GROUP) {
+    const int t = t0 + g;
+    const bool valid = t < m.ntree && !tcoupled[t];
+    const int lo = valid ? m.tree_dofadr[t] : 0, nt = valid ? m.tree_dofnum[t] : 0, cnt = valid ? tcount[t] : 0;
+    const int mydof = lo + l;
+    const bool mine = l < nt;
+    double r[GE_GROUP];
+#pragma unroll
+    for (int j = 0; j < GE_GROUP; j++) {
+      const int a = mine ? m.dof_Mcol[mydof * GE_GROUP + j] : -1;
+      r[j] = mine ? (a >= 0 ? qM[a] : 0.0) : (j == l ? 1.0 : 0.0);
+    }
+    int maxcnt = cnt;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) maxcnt = max(maxcnt, __shfl_xor_sync(FULL, maxcnt, o));
+    NO_UNROLL for (int n = 0; n < maxcnt; n++) {
+      const bool act = n < cnt && l < nt;
+      double J[6] = {0, 0, 0, 0, 0, 0}, tw[6] = {0, 0, 0, 0, 0, 0};
+      if (act) {
+        const int ci = tlist[t * GE_TLIST + n];
+        const double* c = ws + L.con + ci * L.cstride;
+        const int dim = wi[L.i_cdim + ci], t1 = wi[L.i_ct1 + ci], t2 = wi[L.i_ct2 + ci];
+        // sign of my dof in the contact's dof list (chains of both bodies minus their common ancestors) from the per-body
+        // bit masks over the tree-local dof index
+        unsigned m1 = t1 == t ? (unsigned)m.body_chainmask[wi[L.i_cb1 + ci]] : 0u, m2 = t2 == t ? (unsigned)m.body_chainmask[wi[L.i_cb2 + ci]] : 0u;
+        double sgn = ((m2 & ~m1) >> l & 1u) ? 1.0 : (((m1 & ~m2) >> l & 1u) ? -1.0 : 0.0);
+        if (sgn != 0) { jac_column(c, dim, cdof + 6 * mydof, sgn, J); weight_column(c, dim, wi[L.i_cact + ci], J, tw); }
+      }
+#pragma unroll
+      for (int f = 0; f < GE_GROUP; f++) {
+        double h = 0;
+        NO_UNROLL for (int k = 0; k < m.maxdim; k++) h += tw[k] * __shfl_sync(FULL, J[k], gw + f);
+        if (act && l >= f && f < nt && h != 0.0) r[f] += h;
+      }
+    }
+    if (valid) {
+      NO_UNROLL for (int i = 0; i < nsr; i++) {
+        if (!wi[L.i_sract + i]) continue;
+        const int A = wi[L.i_srA + i], B = wi[L.i_srB + i];
+        if (m.dof_treeindex[A] != t) continue;
+        const double D = srv(ws, SR_D, i), ca = srv(ws, SR_CA, i), cb = srv(ws, SR_CB, i);
+        const int a = A - lo, b = B - lo, hi = a > b ? a : b, lw = a > b ? b : a;
+#pragma unroll
+        for (int j = 0; j < GE_GROUP; j++) if (l == a && j == a) r[j] += D * ca * ca;
+        if (B >= 0) {
+#pragma unroll
+          for (int j = 0; j < GE_GROUP; j++) if (l == b && j == b) r[j] += D * cb * cb;
+#pragma unroll
+          for (int j = 0; j < GE_GROUP; j++) if (l == hi && j == lw) r[j] += D * ca * cb;
+        }
+      }
+    }
+    GE_CLK(SC_HESS_TREES);
+    if (valid) group_chol_regs(r, lo, nt, l, gmask, g_, x, -1.0);
+    GE_CLK(SC_CHOL);
+  }
+  gsync();
 }
 
 // x := (M + hdamp * diag(damping))^-1 x  for the block-diagonal (per kinematic tree) mass matrix, through dense per-tree
@@ -414,9 +460,9 @@ __device__ __noinline__ void mass_block_solve(double* ws, double* x, double hdam
   gsync();
 }
 
-// x := -H^-1 g.  Uncoupled trees: 8-lane groups (group_chol_solve).  Coupled trees: right-looking dense Cholesky of the island's block
-// with one whole warp (each lane owns rows lane, lane+32, ... of the block); the warps of a CTA-per-env build take the islands they
-// own (island_owner) concurrently.
+// x := -H^-1 g on the coupled trees (the uncoupled ones are tree_solve's): right-looking dense Cholesky of each island's block with
+// one whole warp (each lane owns rows lane, lane+32, ... of the block); the warps of a CTA-per-env build take the islands they own
+// (island_owner) concurrently.
 __device__ __noinline__ void cholesky_solve(double* ws, int* wi, double* x, const double* g_, int lane) {
   const DevModel& m = c_m; const Layout& L = c_L;
   double* H = wi[L.i_hflag] ? g_hovf[threadIdx.y] : ws + L.H;
@@ -424,16 +470,6 @@ __device__ __noinline__ void cholesky_solve(double* ws, int* wi, double* x, cons
   const int *tcoupled = wi + L.i_tcoupled, *tlist = wi + L.i_tlist;
   bool any_coupled = false;
   for (int t = 0; t < m.ntree; t++) any_coupled |= tcoupled[t] != 0;
-  {
-    const int g = lane / GE_GROUP, l = lane % GE_GROUP;
-    const unsigned gmask = ((1u << GE_GROUP) - 1u) << ((wl / GE_GROUP) * GE_GROUP);
-    for (int t0 = 0; t0 < m.ntree; t0 += GE_LANES / GE_GROUP) {
-      int t = t0 + g;
-      if (t >= m.ntree || tcoupled[t]) continue;  // group-uniform
-      group_chol_solve(H + T_HOFF(tlist, t), m.tree_dofadr[t], m.tree_dofnum[t], l, gmask, g_, x, -1.0);
-    }
-  }
-  gsync();
   if (!any_coupled) return;
   // coupled trees: one dense Cholesky per island block (rows in ascending dof order), rows spread over the lanes of the owner warp.
   // The block-row -> dof lists of the islands are laid out one after the other in the int scratch (the islands partition the

@@ -23,6 +23,9 @@ struct DevModel {
   const double *jnt_pos, *jnt_axis, *jnt_range, *jnt_margin, *jnt_solref, *jnt_solimp;
   const int *dof_bodyid, *dof_jntid, *dof_parentid, *dof_Madr, *dof_subtreenum, *dof_depth, *dof_treeindex, *tree_dofadr, *tree_dofnum, *tree_simple;
   const double *dof_armature, *dof_damping, *dof_invweight0, *tree_Minv;
+  // [nv][GE_GROUP]: index in qM of entry (i, tree_dofadr + j) of dof i's row of its tree's mass block, -1 where that entry is zero
+  // (derived at ge_create from dof_parentid / dof_Madr; used by the register Hessian blocks of ge_hessian.cuh)
+  const int* dof_Mcol;
   const int *geom_type, *geom_bodyid, *geom_meshid;
   const double *geom_pos, *geom_lmat, *geom_size, *geom_rbound, *geom_obbcenter, *geom_obbhalf, *geom_rgba;
   const int *mesh_vertadr, *mesh_vertnum, *mesh_faceadr, *mesh_facenum;

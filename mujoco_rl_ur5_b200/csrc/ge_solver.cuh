@@ -6,7 +6,8 @@
 //   J^T f : one lane per body gathers the wrenches of its contacts, subtree sums over contiguous body ranges,
 //           then one lane per dof takes cdof_d . W_subtree(body_d).
 // Only the Newton Hessian  H = M + J^T D_active J  is formed explicitly (packed lower triangle, skyline Cholesky);
-// the per-contact Jacobian block it needs is rebuilt in registers, one lane per dof of the two kinematic chains.
+// the per-contact Jacobian block it needs is rebuilt in registers, one lane per dof of the two kinematic chains (uncoupled trees:
+// the block itself stays in registers, see ge_hessian.cuh).
 //
 // Stands in for mj_makeConstraint + mj_solNewton behind `sim.step()` (reference: MujocoController.py:379; the
 // scenes set no <option solver=...>, so MuJoCo's default Newton solver and pyramidal cones are in force —
@@ -295,7 +296,8 @@ __device__ __noinline__ int solve_newton(double* ws, int* wi, int lane, int ncon
     if (it == 0) newton_barrier(sync);
     GE_CLK(SC_BARRIER);
     build_hessian(ws, wi, ncon, nsr, lane);
-    GE_CLK(SC_HESSIAN);
+    GE_CLK(SC_HESS_ISLANDS);
+    tree_solve(ws, wi, ncon, nsr, search, grad, lane);
     if (it == 0) newton_barrier(sync);
     GE_CLK(SC_BARRIER);
     cholesky_solve(ws, wi, search, grad, lane);

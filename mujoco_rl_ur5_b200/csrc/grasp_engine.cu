@@ -515,6 +515,7 @@ struct ge_engine {
   Layout lay;
   EnvArrays E;
   void* dblob;       // whole blob on the device
+  int* d_mcol;       // DevModel::dof_Mcol
   std::vector<char> hblob;
   double base_pos[3];
   int64_t launches, substep_launches;
@@ -794,6 +795,19 @@ extern "C" int ge_create(const void* model_blob, size_t nbytes, int n_envs, int 
   if (h->lay.fk_bytes > 227 * 1024) { cudaFree(h->dblob); delete h; return fail(GE_ERR_MODEL, "model too large: kinematics workspace exceeds shared memory"); }
   CK(cudaMalloc(&h->lay.hovf_builds, sizeof(unsigned long long)));
   CK(cudaMemset(h->lay.hovf_builds, 0, sizeof(unsigned long long)));
+  {  // dense qM index table of the tree blocks' rows (DevModel::dof_Mcol): the dof_parentid walk of a row, done once
+    const int *par = (const int*)blob_find(B, "dof_parentid", nullptr), *madr = (const int*)blob_find(B, "dof_Madr", nullptr);
+    const int *tind = (const int*)blob_find(B, "dof_treeindex", nullptr), *tadr = (const int*)blob_find(B, "tree_dofadr", nullptr);
+    std::vector<int> tab((size_t)(m.nv > 0 ? m.nv : 1) * GE_GROUP, -1);
+    for (int i = 0; i < m.nv; i++) {
+      const int lo = tadr[tind[i]];
+      int k = 0;
+      for (int j = i; j >= 0; j = par[j], k++) if (j - lo < GE_GROUP) tab[(size_t)i * GE_GROUP + j - lo] = madr[i] + k;
+    }
+    CK(cudaMalloc(&h->d_mcol, tab.size() * sizeof(int)));
+    CK(cudaMemcpy(h->d_mcol, tab.data(), tab.size() * sizeof(int), cudaMemcpyHostToDevice));
+    m.dof_Mcol = h->d_mcol;
+  }
   CK(cudaMemcpyToSymbol(c_m, &m, sizeof m));
   CK(cudaMemcpyToSymbol(c_L, &h->lay, sizeof(Layout)));
   { int nc = 0; if (const char* ev = getenv("GE_NANCHECK")) nc = atoi(ev) != 0; CK(cudaMemcpyToSymbol(c_nancheck, &nc, sizeof nc)); }
@@ -870,7 +884,7 @@ extern "C" int ge_destroy(ge_handle h) {
   EnvArrays& E = h->E;
   void* ptrs[] = {E.qpos, E.qvel, E.qaccws, E.ctl, E.cmd_mask, E.cmd_maxsteps, E.cmd_steps, E.cmd_result, E.cmd_active, E.cmd_tol, E.prog_phase,
                   E.prog_rot, E.prog_grasp, E.prog_aux, E.prog_info, E.prog_coords, E.prog_table, E.reward, E.status, E.substeps, E.busy_count,
-                  h->d_nout, h->d_dbg, h->dblob, E.gws, E.lock, E.owed, E.done, E.ticket, h->lay.hovf_builds, h->d_check, h->state_scratch};
+                  h->d_nout, h->d_dbg, h->dblob, E.gws, E.lock, E.owed, E.done, E.ticket, h->lay.hovf_builds, h->d_check, h->state_scratch, h->d_mcol};
   for (void* p : ptrs) cudaFree(p);
   render_free(h->rctx);
   delete h;

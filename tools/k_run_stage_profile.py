@@ -18,9 +18,11 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 STAGES = ["PID", "stage_fk", "collision (broad phase, analytic pairs, contact parameters)", "MPR", "stage_rne + stage_crb",
-          "smooth forces + mass solve", "stage_constraints", "Newton (warm start, gradient, directions)", "Hessian build", "Cholesky",
+          "smooth forces + mass solve", "stage_constraints", "Newton (warm start, gradient, directions)",
+          "Hessian: coupling, lists, islands, offsets", "Hessian: M rows", "Hessian: uncoupled trees", "Hessian: islands", "Cholesky",
           "line search", "nt_update", "Euler", "scheduler / program / load / store", "barrier waits"]
-SC_SUBSTEPS, SC_WARM_FK, SC_WARM_RNE_CRB, SC_WARM_MULM, SC_MULM_COLD, SC_NUM = 15, 16, 17, 18, 19, 20
+# the slots behind the stages, in ge_clocks.cuh's order
+SC_SUBSTEPS, SC_WARM_FK, SC_WARM_RNE_CRB, SC_WARM_MULM, SC_MULM_COLD, SC_HESS_BUILDS, SC_HESS_COUPLED, SC_NUM = range(18, 26)
 SLOTS = 4096
 
 
@@ -102,10 +104,15 @@ def main():
     for i, s in enumerate(STAGES):
         print("%-*s" % (w, s) + "".join("%14.0f" % (r["rows"][i] / r["substeps"]) for r in res))
     print("%-*s" % (w, "total") + "".join("%14.0f" % (sum(r["rows"]) / r["substeps"]) for r in res))
+    hess = [STAGES.index(s) for s in STAGES if s.startswith("Hessian")]
+    print("%-*s" % (w, "  of which Hessian build") + "".join("%14.0f" % (sum(r["rows"][i] for i in hess) / r["substeps"]) for r in res))
     print("%-*s" % (w, "  of which first mul_M of Newton") + "".join("%14.0f" % (r["cycles"][SC_MULM_COLD] / r["substeps"]) for r in res))
     for name, i in (("warm stage_fk", SC_WARM_FK), ("warm stage_rne + stage_crb", SC_WARM_RNE_CRB), ("warm mul_M", SC_WARM_MULM)):
         if any(r["cycles"][i] for r in res):
             print("%-*s" % (w, name) + "".join("%14.0f" % (r["cycles"][i] / r["substeps"]) for r in res))
+    print("%-*s" % (w, "Hessian builds per sub-step") + "".join("%14.3f" % (r["cycles"][SC_HESS_BUILDS] / r["substeps"]) for r in res))
+    print("%-*s" % (w, "  share with a coupled tree") + "".join("%14.3f" % (r["cycles"][SC_HESS_COUPLED] / max(r["cycles"][SC_HESS_BUILDS], 1))
+                                                                 for r in res))
     print("%-*s" % (w, "sub-steps / s (profile build)") + "".join("%14.0f" % r["substeps_per_s"] for r in res))
 
 
